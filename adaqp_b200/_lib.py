@@ -20,7 +20,9 @@ i32 = C.c_int32
 u64 = C.c_uint64
 u32 = C.c_uint32
 
-ADAQP_ABI_VERSION = 2
+ADAQP_ABI_VERSION = 3
+MAX_PARTS = 64           # ADAQP_MAX_PARTS
+LP_HUB_DEGREE = 256      # ADAQP_LP_HUB_DEGREE
 IPC_HANDLE_BYTES = 64
 ST_OK, ST_FLAG_TIMEOUT, ST_ACK_TIMEOUT = 0, 1, 2
 
@@ -94,6 +96,16 @@ SYMBOLS = {
                                         c_void_p, i32, c_void_p]),
     "adaqp_gather_rows_f32": (C.c_int, [c_void_p, i64, c_void_p, i64, i32, c_void_p, i64,
                                         c_void_p]),
+    "adaqp_lp_rate_clusters": (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, i64, c_void_p, c_void_p, i64,
+                                         c_void_p, i64, c_void_p, i32, u64, u32, C.c_int, c_void_p, c_void_p,
+                                         c_void_p, c_void_p]),
+    "adaqp_lp_rate_blocks": (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, i64, c_void_p, c_void_p, i32, i64,
+                                       u64, u32, C.c_int, C.c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "adaqp_lp_apply": (C.c_int, [c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, i64, c_void_p,
+                                 c_void_p]),
+    "adaqp_lp_rebalance_select": (C.c_int, [c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p, i64, c_void_p,
+                                            c_void_p]),
+    "adaqp_contract_edges": (C.c_int, [c_void_p, c_void_p, i64, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -139,7 +139,8 @@ def load_rank_layout(part_dir: str, dataset: str, model_type: DistGNNType) -> Ra
     # partition path cannot silently train on random data under the real dataset's name.
     if os.environ.get("ADAQP_SYNTHETIC", "0") != "1":
         raise FileNotFoundError(
-            f"no partition file {path}. Convert real partitions with tools/convert_dgl_partition.py, or set "
+            f"no partition file {path}. Partition a dataset with graph_partition.py, convert DGL partitions with "
+            f"tools/convert_dgl_partition.py, or set "
             f"ADAQP_SYNTHETIC=1 to train on synthetic partitions of the dataset's shape (config `synthetic:`).")
     scale = float(os.environ.get("ADAQP_SYNTH_SCALE", "1.0"))
     spec = spec_from_config(_load_config(dataset), W, scale)

@@ -3,15 +3,19 @@
 Pipeline of the reference's GraphEngine.__init__ (AdaQP/manager/graphEngine.py:54-76):
 convert_partition -> get_send_recv_idx_scores -> reorder_graph -> convert_send_idx
 (-> decompose_graph), restated DGL-free on numpy CSR.  `prepare_rank` is the multi-process
-form (collectives supplied by the caller), `prepare_all_in_process` wires W ranks inside
-one process for tests, smoke() and the single-GPU loopback bench.
+form (collectives supplied by the caller), `layouts_from_raw` wires W ranks inside one process
+(synthetic partitions for tests, smoke() and the single-GPU loopback bench; real partitions from
+`raw_partitions` or tools/convert_dgl_partition.py).
 """
 from __future__ import annotations
 
+import json
+import os
 from dataclasses import dataclass
 from typing import Callable, Dict, List, Tuple
 
 import numpy as np
+import scipy.sparse as sp
 
 from ..helper import DistGNNType
 from . import conversion as cv
@@ -70,6 +74,18 @@ def prepare_rank(spec: SynthSpec, rank: int, model_type: DistGNNType,
     return _finish(raw, recv_idx, send_ids, scores)
 
 
+def layouts_from_raw(raws: List[RawPartition], model_type: DistGNNType) -> List[RankLayout]:
+    """halo_requests -> send_side -> reorder / convert_send_idx / decompose for all ranks in one process (the
+    reference does the two exchanges with all_gather_object, processing.py:65-71).  `raws` carry global degrees."""
+    rr = [cv.halo_requests(r, model_type) for r in raws]
+    all_requests = [x[1] for x in rr]
+    out = []
+    for r in range(len(raws)):
+        send_ids, scores = cv.send_side(r, all_requests)
+        out.append(_finish(raws[r], rr[r][0], send_ids, scores))
+    return out
+
+
 def prepare_all_in_process(spec: SynthSpec, model_type: DistGNNType = DistGNNType.DistGCN) -> List[RankLayout]:
     W = spec.num_parts
     raws = [build_raw_partition(spec, r) for r in range(W)]
@@ -77,10 +93,59 @@ def prepare_all_in_process(spec: SynthSpec, model_type: DistGNNType = DistGNNTyp
     starts = block_starts(spec)
     for r in raws:
         attach_global_degrees(r, degs, starts)
-    rr = [cv.halo_requests(r, model_type) for r in raws]
-    all_requests = [x[1] for x in rr]
-    out = []
-    for r in range(W):
-        send_ids, scores = cv.send_side(r, all_requests)
-        out.append(_finish(raws[r], rr[r][0], send_ids, scores))
-    return out
+    return layouts_from_raw(raws, model_type)
+
+
+def raw_partitions(graph, part: np.ndarray) -> List[RawPartition]:
+    """Cut a global graph (helper.dataset.GlobalGraph: symmetric CSR, node data) along `part`.
+
+    Nodes are relabelled so that block p owns a contiguous range of global ids, ascending original id within
+    the block (DGL's reshuffle).  Rank p keeps the in-edges of its inner nodes, the ids and owners of its halo
+    nodes, its slices of features / labels / masks and the global degrees (CSR row lengths) of all its nodes."""
+    part = np.asarray(part, np.int64)
+    n = graph.indptr.size - 1
+    assert part.shape == (n,), (part.shape, n)
+    W = int(part.max()) + 1
+    old_of_new = np.argsort(part, kind="stable")
+    new_of_old = np.empty(n, np.int64)
+    new_of_old[old_of_new] = np.arange(n)
+    starts = np.concatenate([[0], np.cumsum(np.bincount(part, minlength=W))]).astype(np.int64)
+    deg = np.diff(graph.indptr).astype(np.int64)
+    A = sp.csr_matrix((np.ones(graph.indices.size, np.int8), graph.indices, graph.indptr), shape=(n, n))
+    raws = []
+    for p in range(W):
+        g0, g1 = int(starts[p]), int(starts[p + 1])
+        ids = old_of_new[g0:g1]
+        rows = A[ids]
+        src = new_of_old[rows.indices]
+        inner = (src >= g0) & (src < g1)
+        halo_gid = np.unique(src[~inner])
+        local = np.empty(src.size, np.int64)
+        local[inner] = src[inner] - g0
+        local[~inner] = (g1 - g0) + np.searchsorted(halo_gid, src[~inner])
+        B = sp.csr_matrix((np.ones(src.size, np.int8), local, rows.indptr), shape=(g1 - g0, g1 - g0 + halo_gid.size))
+        B.sort_indices()
+        d = deg[np.concatenate([ids, old_of_new[halo_gid]])]
+        raws.append(RawPartition(
+            rank=p, num_parts=W, n_inner=g1 - g0, inner_start=g0, starts=starts, indptr=B.indptr.astype(np.int64),
+            indices=B.indices.astype(np.int32), halo_gid=halo_gid.astype(np.int64),
+            halo_part=(np.searchsorted(starts, halo_gid, side="right") - 1).astype(np.int32),
+            feat=graph.feat[ids], label=graph.label[ids], train_mask=graph.train_mask[ids],
+            val_mask=graph.val_mask[ids], test_mask=graph.test_mask[ids], in_degrees=d, out_degrees=d.copy()))
+    return raws
+
+
+def save_partition_book(part: np.ndarray, part_dir: str, dataset: str, header: dict) -> str:
+    """`<part_dir>/<dataset>/<W>part/partition_book.npz`: the block of every original node id plus a JSON header
+    (seed, k, edge cut, block sizes, halo rows ...); plain arrays, nothing is unpickled on load."""
+    d = f"{part_dir}/{dataset}/{int(header['k'])}part"
+    os.makedirs(d, exist_ok=True)
+    path = f"{d}/partition_book.npz"
+    np.savez_compressed(path, part=np.ascontiguousarray(part, np.int32),
+                        header_json=np.frombuffer(json.dumps(header).encode("utf-8"), dtype=np.uint8))
+    return path
+
+
+def read_partition_book(path: str):
+    z = np.load(path, allow_pickle=False)
+    return z["part"], json.loads(bytes(z["header_json"]).decode("utf-8"))

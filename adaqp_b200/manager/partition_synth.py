@@ -277,3 +277,25 @@ def build_all_partitions(spec: SynthSpec) -> List[RawPartition]:
     for r in raws:
         attach_global_degrees(r, degs, starts)
     return raws
+
+
+def global_graph(spec: SynthSpec):
+    """The generator's whole graph as one helper.dataset.GlobalGraph (symmetric CSR with self-loops, node data)
+    and its planted blocks `part` -- the input graph_partition.py would see for a dataset of this shape."""
+    from ..helper.dataset import GlobalGraph
+    raws = build_all_partitions(spec)
+    rows, cols = [], []
+    for r in raws:
+        rows.append(r.inner_start + np.repeat(np.arange(r.n_inner, dtype=np.int64), np.diff(r.indptr)))
+        loc = r.indices.astype(np.int64)
+        halo = r.halo_gid[np.maximum(loc - r.n_inner, 0)] if r.n_halo else loc
+        cols.append(np.where(loc < r.n_inner, loc + r.inner_start, halo))
+    n = spec.num_nodes
+    row = np.concatenate(rows)
+    A = sp.csr_matrix((np.ones(row.size, np.int8), (row, np.concatenate(cols))), shape=(n, n))
+    A.sort_indices()
+    cat = lambda f: np.concatenate([getattr(r, f) for r in raws])  # noqa: E731
+    g = GlobalGraph(name=spec.name, indptr=A.indptr.astype(np.int64), indices=A.indices.astype(np.int32),
+                    feat=cat("feat"), label=cat("label"), train_mask=cat("train_mask"), val_mask=cat("val_mask"),
+                    test_mask=cat("test_mask"))
+    return g, np.concatenate([np.full(r.n_inner, r.rank, np.int32) for r in raws])

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define ADAQP_ABI_VERSION 2
+#define ADAQP_ABI_VERSION 3
 
 #define ADAQP_EINVAL (-1)   /* bad argument (bits not in {1,2,4,8}, negative size ...) */
 #define ADAQP_EALIGN (-2)   /* pointer alignment requirement violated */
@@ -269,6 +269,46 @@ int adaqp_ln_relu_bwd_f32(const float *dy, int64_t lddy, const float *x, int64_t
 /* Row gather out[i] = x[idx[i]] (copy-buffer fills of ops.py:159-164; API parity only). */
 int adaqp_gather_rows_f32(const float *x, int64_t ld, const int64_t *idx, int64_t n,
                           int32_t F, float *out, int64_t ldo, void *stream);
+
+/* ------------------------------------------------------------ graph partitioning
+ * Multilevel label-propagation k-way partitioning (csrc/partition.cu, level driver and host initial
+ * partition in adaqp_b200/partition.py): replaces dgl.distributed.partition_graph(graph, ..., num_hops=1,
+ * balance_edges=False), i.e. METIS, at AdaQP/helper/partition.py:71-72.  Graphs are symmetric CSR without
+ * self-loops: int64 indptr[n+1], int32 indices, int32 edge weights ew and vertex weights vw.  Labels are int32;
+ * label weights (lw / bw) are int64.  One sub-round (round, sub) moves only the vertices v with
+ * h(seed, round, v) & 1 == sub, h = splitmix64 mix (DESIGN.md, "Graph partitioning").  Every rating kernel
+ * writes, per vertex, tgt[v] (proposed label, -1 = none), gain[v] = rho(tgt) - rho(label[v]) and
+ * hkey[v] = h(seed, round, v) >> 1, the order key of the apply step. */
+#define ADAQP_MAX_PARTS 64          /* the exchange's channel limit */
+#define ADAQP_LP_HUB_DEGREE 256     /* clustering: vertices of larger degree are rated by the hub path */
+
+/* Clustering sub-round rating: candidate labels are the neighbours' labels c with lw[c] + vw[v] <= cap;
+ * only positive gains are proposed.  Labels are < n.  Vertices of degree > ADAQP_LP_HUB_DEGREE must all be listed
+ * in hubs[n_hubs]; they are rated by min(n_hubs, hub_ctas) CTAs, CTA b counting in the dense row
+ * hub_scratch[b * n .. (b + 1) * n), which must be zero on entry and is left zero. */
+int adaqp_lp_rate_clusters(const int64_t *indptr, const int32_t *indices, const int32_t *ew, const int32_t *vw,
+                           int64_t n, const int32_t *label, const int64_t *lw, int64_t cap, const int32_t *hubs,
+                           int64_t n_hubs, uint32_t *hub_scratch, int32_t hub_ctas, uint64_t seed, uint32_t round, int sub,
+                           int32_t *tgt, int64_t *gain, int64_t *hkey, void *stream);
+/* k-way rating, 1 <= k <= ADAQP_MAX_PARTS.  mode 0: refinement sub-round (positive gains only);
+ * mode 1: rebalancing, every vertex of a block with bw > cap proposes its best block with room, any gain. */
+int adaqp_lp_rate_blocks(const int64_t *indptr, const int32_t *indices, const int32_t *ew, const int32_t *vw, int64_t n,
+                         const int32_t *part, const int64_t *bw, int32_t k, int64_t cap, uint64_t seed, uint32_t round,
+                         int sub, int mode, int32_t *tgt, int64_t *gain, int64_t *hkey, void *stream);
+/* Apply: order[n_prop] = proposing vertices sorted by (tgt asc, gain desc, hkey asc, v asc); csum = inclusive
+ * prefix sum of vw[order].  Per target b the longest prefix with lw[b] + prefix weight <= cap is accepted:
+ * label[v] = b and dlw[b] += vw[v], dlw[old label] -= vw[v] (the caller adds dlw to lw). */
+int adaqp_lp_apply(const int32_t *order, int64_t n_prop, const int64_t *csum, const int32_t *tgt, const int32_t *vw,
+                   int32_t *label, const int64_t *lw, int64_t cap, int64_t *dlw, void *stream);
+/* Rebalancing, source side: order = proposals of mode 1 sorted by (part asc, gain desc, hkey asc, v asc), csum as
+ * above.  Per over-full block keeps the shortest prefix whose weight covers bw - cap and sets tgt[v] = -1 for the
+ * rest; the kept proposals then go through adaqp_lp_apply. */
+int adaqp_lp_rebalance_select(const int32_t *order, int64_t n_prop, const int64_t *csum, const int32_t *part,
+                              const int32_t *vw, const int64_t *bw, int64_t cap, int32_t *tgt, void *stream);
+/* Contraction: key[e] = (int64)cid[v] << 32 | cid[indices[e]] for every edge e of row v, INT64_MAX when both
+ * ends are in the same cluster (the caller sorts the keys and sums the weights of equal keys). */
+int adaqp_contract_edges(const int64_t *indptr, const int32_t *indices, int64_t n, const int32_t *cid, int64_t *key,
+                         void *stream);
 
 #ifdef __cplusplus
 }

@@ -74,16 +74,9 @@ def raw_from_arrays(a: Dict[str, np.ndarray], rank: int, world: int):
 
 
 def convert(raws: List, model_type) -> List:
-    """halo_requests -> send_side -> reorder / convert_send_idx / decompose for all ranks in one process
-    (the reference does the two exchanges with all_gather_object, processing.py:65-71)."""
-    from adaqp_b200.manager import conversion as cv
-    from adaqp_b200.manager.layout import _finish
-    rr = [cv.halo_requests(r, model_type) for r in raws]
-    out = []
-    for r in range(len(raws)):
-        send_ids, scores = cv.send_side(r, [x[1] for x in rr])
-        out.append(_finish(raws[r], rr[r][0], send_ids, scores))
-    return out
+    """The package's shared chain (manager.layout.layouts_from_raw), as graph_partition.py runs it."""
+    from adaqp_b200.manager.layout import layouts_from_raw
+    return layouts_from_raw(raws, model_type)
 
 
 def main():
