@@ -20,7 +20,7 @@ i32 = C.c_int32
 u64 = C.c_uint64
 u32 = C.c_uint32
 
-ADAQP_ABI_VERSION = 3
+ADAQP_ABI_VERSION = 4
 MAX_PARTS = 64           # ADAQP_MAX_PARTS
 LP_HUB_DEGREE = 256      # ADAQP_LP_HUB_DEGREE
 IPC_HANDLE_BYTES = 64
@@ -106,6 +106,12 @@ SYMBOLS = {
     "adaqp_lp_rebalance_select": (C.c_int, [c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p, i64, c_void_p,
                                             c_void_p]),
     "adaqp_contract_edges": (C.c_int, [c_void_p, c_void_p, i64, c_void_p, c_void_p, c_void_p]),
+    "adaqp_gat_scores_f32": (C.c_int, [c_void_p, i64, i64, i32, i32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "adaqp_gat_fwd_f32": (C.c_int, [c_void_p, c_void_p, i64, c_void_p, i64, c_void_p, i64, c_void_p, c_void_p, c_void_p,
+                                    i32, i32, i64, i64, c_void_p, i64, c_void_p, c_void_p]),
+    "adaqp_gat_bwd_f32": (C.c_int, [c_void_p, c_void_p, i64, c_void_p, i64, c_void_p, i64, c_void_p, i64, c_void_p, i64,
+                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, i32, i32, i64, i64,
+                                    c_void_p, i64, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -20,6 +20,7 @@ from torch import Tensor
 
 from ..communicator import BITS_SET
 from ..communicator import Communicator as comm
+from ..communicator.p2p import quantisable
 from ..helper import BitType
 from ..manager import GraphEngine as engine
 from . import solver
@@ -40,8 +41,15 @@ class Assigner(object):
 
     def __init__(self, feat_dim: int, hidden_dim: int, num_layers: int, num_data: int, scheme: str,
                  uniform_assign_bits: int, scores: Dict[int, Tuple[Tensor, Tensor]], group_size: int,
-                 coe_lambda: float, assign_cycle: int = None, warmup: int = 1):
+                 coe_lambda: float, assign_cycle: int = None, warmup: int = 1, key_dims: Dict[str, int] = None):
         assert scheme in ASSIGNMENT_SCHEME, f"assignment scheme {scheme} is not supported"
+        # keys that travel quantised and their row widths: by default forward0..L-1 / backward1..L-1 with layer 0
+        # feat_dim wide; a model with its own exchange (GAT) passes every key's real width
+        if key_dims is None:
+            self.key_dims = {k: (feat_dim if k.endswith("0") else hidden_dim) for k in _layer_keys(num_layers)}
+        else:
+            self.key_dims = {k: int(v) for k, v in key_dims.items() if quantisable(k)}
+        self.keys = list(self.key_dims)
         self.bits_set = torch.tensor(BITS_SET, dtype=torch.int32)
         self.bits_cost = torch.tensor([1 / (2 ** b - 1) ** 2 for b in BITS_SET], dtype=torch.float32)
         self.feat_dim, self.hidden_dim, self.num_layers = feat_dim, hidden_dim, num_layers
@@ -85,11 +93,11 @@ class Assigner(object):
     # ---- simple schemes (:95-120) ------------------------------------------------------------
     def _get_uniform_assignment(self, send_idx):
         return {key: {pid: torch.full((hi - lo,), self.uniform_assign_bits, dtype=torch.int32)
-                      for pid, (lo, hi) in send_idx.items()} for key in _layer_keys(self.num_layers)}
+                      for pid, (lo, hi) in send_idx.items()} for key in self.keys}
 
     def _get_random_sampling_assignment(self, send_idx):
         out = {}
-        for key in _layer_keys(self.num_layers):
+        for key in self.keys:
             out[key] = {}
             for pid, (lo, hi) in send_idx.items():
                 pick = torch.multinomial(self.sample_rate, hi - lo, replacement=True)
@@ -98,7 +106,7 @@ class Assigner(object):
 
     # ---- adaptive scheme (:128-304) -------------------------------------------------------------
     def init_traced_data(self, num_layers: int):
-        for key in _layer_keys(num_layers):
+        for key in self.keys:
             self.traced_layer_data[key] = 0.0
 
     def slice_traced_data(self, send_idx):
@@ -115,7 +123,7 @@ class Assigner(object):
         var_matrix, comm_matrix, idx_set = {}, {}, {}
         for key, per_peer in self.traced_layer_data.items():
             var_matrix[key], comm_matrix[key], idx_set[key] = {}, {}, {}
-            dim = feats_dim if "0" in key else hidden_dim
+            dim = self.key_dims[key]
             for pid, traced in per_peer.items():
                 agg = scores[pid][0] if "forward" in key else scores[pid][1]
                 assert agg.shape == traced.shape

@@ -55,7 +55,9 @@ def _profile_p2p(feat_dim, hidden_dim, num_data, warmup, reps: int = 5):
     rank = comm.get_rank()
     dev = comm.ctx.device
     n_inner = engine.ctx.num_inner
-    keys = [("forward0", feat_dim), ("forward1", hidden_dim)] if len(ex.buffer_shape) > 1 else [("forward0", feat_dim)]
+    # the real exchanged widths of the first two forward keys (feat_dim / hidden_dim for GCN and SAGE; GAT exchanges
+    # the projected rows, hidden_dim wide from layer 0 on)
+    keys = [(k, ex.dims[k]) for k in ("forward0", "forward1") if k in ex.dims]
     xs = {k: torch.relu(torch.randn(n_inner, F, device=dev)) for k, F in keys}
     S = int(sum(hi - lo for lo, hi in ex.send_idx.values()))
     mbs, ts = [], []

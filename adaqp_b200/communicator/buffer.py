@@ -44,9 +44,10 @@ class CommBuffer(object):
     def __init__(self, buffer_shape: List[int], send_idx: Dict[int, Tuple[int, int]],
                  recv_idx: Basic_Buffer_Type, bit_type: BitType, device: torch.device,
                  transport: str = None, total_send_idx: Tensor = None, num_remote: int = None,
-                 exchange: "p2p.PeerExchange" = None):
+                 exchange: "p2p.PeerExchange" = None, key_dims: Dict[str, int] = None):
         assert bit_type in [BitType.FULL, BitType.QUANT], f"bit_type should be either FULL or QUANT, but got {bit_type}"
         self.buffer_shape = [int(x) for x in buffer_shape]
+        self.key_dims = key_dims          # per-key exchange widths (GAT); None = the layer keys of buffer_shape
         self.device = torch.device(device)
         self.bit_type = bit_type
         self.transport = transport or ("p2p" if self.device.type == "cuda" else "gloo")
@@ -72,7 +73,7 @@ class CommBuffer(object):
             total_send_idx, num_remote = engine.ctx.total_send_idx, engine.ctx.num_remove
         rank, W = dist.get_rank(), dist.get_world_size()
         ex = p2p.PeerExchange(rank, W, self.device, self.buffer_shape, self.send_idx, self.recv_idx,
-                              total_send_idx, num_remote)
+                              total_send_idx, num_remote, key_dims=self.key_dims)
         metas = [None] * W
         dist.all_gather_object(metas, ex.local_meta())
         slab = ex.allocate(metas)

@@ -46,6 +46,31 @@ def key_dim(key: str, buffer_shape: Sequence[int]) -> int:
     return int(buffer_shape[int(key[-1])])   # buffer.py:63,201: layer index = last character
 
 
+def attn_keys(layer: int) -> Tuple[str, str]:
+    """fp32 keys of GAT's per-row attention scalars: el rows with the forward exchange, [er | lse | s] rows with the
+    backward exchange.  Training and evaluation never have the same key in flight, so both use them."""
+    return f"attn_fwd{layer}", f"attn_bwd{layer}"
+
+
+def gat_key_dims(widths: Sequence[int], heads: Sequence[int]) -> Dict[str, int]:
+    """Exchange keys and widths of a GAT model whose layer l exchanges rows of z_l (width widths[l], heads[l] heads):
+    test / forward / backward keys of every layer (backward0 included: dW_0 needs the gradient of remote
+    destinations), then the attention keys."""
+    L = len(widths)
+    dims = {f"test{i}": int(widths[i]) for i in range(L)}
+    dims.update({f"forward{i}": int(widths[i]) for i in range(L)})
+    dims.update({f"backward{i}": int(widths[i]) for i in range(L)})
+    for i in range(L):
+        fwd, bwd = attn_keys(i)
+        dims[fwd], dims[bwd] = int(heads[i]), 3 * int(heads[i])
+    return dims
+
+
+def quantisable(key: str) -> bool:
+    """Keys that may travel quantised (training exchanges of layer rows); test and attention keys are fp32."""
+    return key.startswith(("forward", "backward"))
+
+
 def qsize(n: int, bits: int, F: int) -> int:
     """buffer.py:181-186."""
     wpt = 8 // bits
@@ -90,7 +115,7 @@ class SlabLayout:
         off = _up(off)
         for k in keys:
             F = dims[k]
-            if not k.startswith("test"):
+            if quantisable(k):
                 for p in sorted(recv_rows):
                     n = recv_rows[p]
                     L.qdata_off[(k, p)] = off
@@ -276,16 +301,22 @@ class PeerExchange:
     send_idx / recv_idx / total_send_idx follow the reference's contract
     (conversion.py:92-106, processing.py:53-60).  `gather(obj) -> list` is the control
     plane all_gather (comm.all_gather_any in multi-process runs; tests wire ranks
-    in-process through `connect`)."""
+    in-process through `connect`).  `key_dims` (ordered key -> row width, e.g. gat_key_dims) replaces the
+    default keys of layer_keys with widths from buffer_shape."""
 
     def __init__(self, rank: int, world_size: int, device: torch.device, buffer_shape: Sequence[int],
                  send_idx: Dict[int, Tuple[int, int]], recv_idx: Dict[int, torch.Tensor],
-                 total_send_idx: torch.Tensor, num_remote: int, timeout_ns: int = DEFAULT_TIMEOUT_NS):
+                 total_send_idx: torch.Tensor, num_remote: int, timeout_ns: int = DEFAULT_TIMEOUT_NS,
+                 key_dims: Optional[Dict[str, int]] = None):
         self.rank, self.world_size, self.device = rank, world_size, torch.device(device)
         self.buffer_shape = [int(x) for x in buffer_shape]
         self.num_layers = len(self.buffer_shape)
-        self.keys = layer_keys(self.num_layers)
-        self.dims = {k: key_dim(k, self.buffer_shape) for k in self.keys}
+        if key_dims is None:
+            self.keys = layer_keys(self.num_layers)
+            self.dims = {k: key_dim(k, self.buffer_shape) for k in self.keys}
+        else:
+            self.keys = list(key_dims)
+            self.dims = {k: int(v) for k, v in key_dims.items()}
         self.send_idx = {int(p): (int(lo), int(hi)) for p, (lo, hi) in send_idx.items()}
         self.recv_idx = {int(p): torch.as_tensor(v).cpu().numpy().astype(np.int64) for p, v in recv_idx.items()}
         self.total_send_idx = torch.as_tensor(total_send_idx).cpu().numpy().astype(np.int64)

@@ -43,6 +43,24 @@ AdaqpOptions &adaqp_options();
         }                                                                    \
     } while (0)
 
+// ---------------------------------------------------------------- frontier row scheduler
+// Row counter of the frontier scheduler: {next_row, finished CTAs}.  The last CTA to finish puts both
+// words back to zero, so a launch needs no memset node and one counter pair per (device, stream)
+// can never be shared by two launches that are in flight together.
+__device__ __forceinline__ void frontier_release(unsigned long long *counter) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const unsigned long long prev = atomicAdd(counter + 1, 1ull);
+        if (prev == (unsigned long long)gridDim.x - 1ull) {
+            counter[0] = 0ull;
+            counter[1] = 0ull;
+            __threadfence();
+        }
+    }
+}
+// The counter pair of (device, stream), allocated zeroed on first use (spmm.cu).
+unsigned long long *adaqp_frontier_counter(int dev, cudaStream_t s);
+
 // ---------------------------------------------------------------- Philox
 // Philox4x32-10 exactly as curand's curand_Philox4x32_10 (curand_philox4x32_x.h):
 // counter (x,y) = Philox offset / 4, (z,w) = subsequence, key = seed.

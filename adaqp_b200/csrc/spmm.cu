@@ -61,21 +61,6 @@ template <> struct Vec<1> {
     static __device__ __forceinline__ void store_cs(float *p, const float (&v)[1]) { __stcs(p, v[0]); }
 };
 
-// Row counter of the frontier scheduler: {next_row, finished CTAs}.  The last CTA to finish puts both
-// words back to zero, so a launch needs no memset node and one counter pair per (device, stream)
-// can never be shared by two launches that are in flight together.
-__device__ __forceinline__ void frontier_release(unsigned long long *counter) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        const unsigned long long prev = atomicAdd(counter + 1, 1ull);
-        if (prev == (unsigned long long)gridDim.x - 1ull) {
-            counter[0] = 0ull;
-            counter[1] = 0ull;
-            __threadfence();
-        }
-    }
-}
-
 template <int VEC, int CHUNKS>
 __global__ void __launch_bounds__(kThreads)
 spmm_csr_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ indices,
@@ -629,6 +614,8 @@ unsigned long long *frontier_counter(int dev, cudaStream_t s) {
 }
 
 }  // namespace
+
+unsigned long long *adaqp_frontier_counter(int dev, cudaStream_t s) { return frontier_counter(dev, s); }
 
 extern "C" {
 

@@ -29,8 +29,9 @@ def graph_patition_store(dataset: str, partition_size: int, raw_dir: str = "data
     from adaqp_b200.manager.graphEngine import save_rank_layout
     from adaqp_b200.manager.layout import layouts_from_raw, raw_partitions, save_partition_book
 
-    if model_name not in ("gcn", "sage"):
-        raise ValueError(f"model_name must be gcn or sage, got {model_name}")
+    MODELS = {"gcn": DistGNNType.DistGCN, "sage": DistGNNType.DistSAGE, "gat": DistGNNType.DistGAT}
+    if model_name not in MODELS:
+        raise ValueError(f"model_name must be one of {sorted(MODELS)}, got {model_name}")
     if not torch.cuda.is_available():
         raise RuntimeError("graph_partition.py partitions on the GPU and no CUDA device is visible")
     times = {}
@@ -41,7 +42,7 @@ def graph_patition_store(dataset: str, partition_size: int, raw_dir: str = "data
     info = {}
     part = gp.partition(graph.indptr, graph.indices, partition_size, seed=seed, info=info)
     t0 = time.perf_counter()
-    model = DistGNNType.DistGCN if model_name == "gcn" else DistGNNType.DistSAGE
+    model = MODELS[model_name]
     layouts = layouts_from_raw(raw_partitions(graph, part), model)
     times["layout"] = time.perf_counter() - t0
     t0 = time.perf_counter()

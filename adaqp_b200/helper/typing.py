@@ -9,6 +9,7 @@ import enum
 class DistGNNType(enum.Enum):
     DistGCN = 0
     DistSAGE = 1
+    DistGAT = 2     # extension beyond the reference
 
 
 @enum.unique

@@ -1,2 +1,3 @@
 from .distGCN import DistGCN  # noqa: F401
 from .distSAGE import DistSAGE  # noqa: F401
+from .distGAT import DistGAT  # noqa: F401

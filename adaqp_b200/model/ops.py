@@ -17,7 +17,9 @@ import torch
 from torch import Tensor
 from torch.autograd import Function
 
+from .. import gat
 from ..communicator import Communicator as comm
+from ..communicator.p2p import attn_keys
 from ..helper import BitType, ProprogationMode
 from ..manager import DecompGraph
 from ..manager import GraphEngine as engine
@@ -245,3 +247,121 @@ def decomposed_graph_propagation(ctx, local_messages: Tensor, graph, layer: int,
     pend.release()
     local_messages.record_stream(side)
     return _finish(ctx, out, layer, mode)
+
+
+# ---------------------------------------------------------------- GAT
+def _gat_exchange(rows: Tensor, name: str, is_train: bool, scalars: Tensor, aux_key: str, stream=None):
+    """Exchange the boundary rows of one layer key (quantised per mode, as halo_exchange does for GCN / SAGE) and
+    their per-row attention scalars in fp32 on `aux_key`: both ranks must compute the softmax from identical
+    scalars.  Returns (pending row exchange, received scalar rows [num_remote, width])."""
+    ex = comm.ctx.comm_buffer.p2p
+    ex.post_send_fp(aux_key, scalars, stream=stream)
+    pend = halo_exchange(rows, name, is_train, stream=stream)
+    return pend, ex.complete_recv_fp(aux_key, stream=stream)
+
+
+def _gat_release(pend, aux_key: str):
+    """After the last consumer of the received rows has been enqueued on the current stream."""
+    pend.release()
+    comm.ctx.comm_buffer.p2p.release_fp(aux_key)
+
+
+def _gat_propagate(name: str, quant: bool, rows: Tensor, scalars: Tensor, aux_key: str, is_train: bool, aggregate):
+    """Exchange + aggregation skeleton of full_graph_propagation / decomposed_graph_propagation for GAT:
+    aggregate(lo, hi, halo_rows, halo_scalars) runs the kernel over inner rows [lo, hi).  Central rows have no halo
+    neighbour in either direction, so in the overlapped mode they run while the exchange is in flight; the
+    marginal rows run in one pass once it has landed (their softmax spans local and halo sources)."""
+    eng, timer = engine.ctx, engine.ctx.timer
+    comm_name = f"{name}_quantization" if quant else f"{name}_communication"
+    if not eng.use_parallel:
+        with timer.record_events(comm_name):
+            pend, aux_halo = _gat_exchange(rows, name, is_train, scalars, aux_key)
+        with timer.record_events(f"{name}_full_aggregation"):
+            kept = aggregate(0, eng.num_inner, pend.halo, aux_halo)
+        _gat_release(pend, aux_key)
+        return kept
+    main, side = torch.cuda.current_stream(), eng.marginal_stream
+    ready = torch.cuda.Event()
+    ready.record(main)                       # rows and scalars are produced on the default stream
+    side.wait_event(ready)
+    with timer.record_events(comm_name, stream=side):
+        pend, aux_halo = _gat_exchange(rows, name, is_train, scalars, aux_key, stream=side)
+    landed = torch.cuda.Event(enable_timing=True)
+    landed.record(side)
+    nc = eng.num_central
+    with timer.record_events(f"{name}_central_aggregation"):
+        aggregate(0, nc, None, None)
+    central_done = torch.cuda.Event(enable_timing=True)
+    central_done.record(main)
+    timer.record_exposed(name, central_done, landed)
+    main.wait_event(landed)
+    with timer.record_events(f"{name}_marginal_aggregation"):
+        kept = aggregate(nc, eng.num_inner, pend.halo, aux_halo)
+    _gat_release(pend, aux_key)
+    rows.record_stream(side)
+    scalars.record_stream(side)
+    return kept
+
+
+class DistAggGAT(Function):
+    """Attention aggregation of local + remote neighbours for GAT (an extension beyond the reference).
+
+    forward(z, a_l, a_r, graph, layer, is_train, heads) -> out: the exchange moves the projected rows z (key
+    forward{l}, quantised per mode; test{l} in evaluation) and each row's el in fp32 (attn_fwd{l}); the received
+    halo z / el are copied out of the slab because the backward pass needs them.  backward exchanges dL/dout
+    (backward{l}) and each row's [er | lse | s] in fp32 (attn_bwd{l}), then gat_bwd gives dz, del and der; da_l /
+    da_r are deterministic torch reductions.  p2p transport only.  The layer-0 evaluation cache never applies: the
+    exchanged rows are z, not the input features."""
+
+    @staticmethod
+    def forward(ctx, z: Tensor, a_l: Tensor, a_r: Tensor, graph, layer: int, is_train: bool, heads: int) -> Tensor:
+        if comm.ctx.transport != "p2p":
+            raise NotImplementedError("GAT runs on the p2p transport only (not the CPU gloo plumbing mode)")
+        eng = engine.ctx
+        z = z.contiguous()
+        n, F = z.shape
+        el, er = gat.scores(z, a_l, a_r, heads)
+        g = graph.full if isinstance(graph, DecompGraph) else graph
+        out = z.new_empty((n, F))
+        lse = z.new_empty((n, heads))
+        fwd_key, _ = attn_keys(layer)
+
+        def aggregate(lo, hi, z_halo, el_halo):
+            if z_halo is not None and is_train:          # kept for the backward pass; the slab rows are reused
+                z_halo, el_halo = z_halo.clone(), el_halo.clone()
+            gat.forward(g, z, z_halo, el, el_halo, er, heads, lo, hi, out[lo:hi], lse[lo:hi])
+            return z_halo, el_halo
+
+        quant = eng.bit_type == BitType.QUANT and is_train
+        z_halo, el_halo = _gat_propagate(f"forward{layer}", quant, z, el, fwd_key, is_train, aggregate)
+        if is_train:
+            ctx.save_for_backward(z, z_halo, el, el_halo, er, out, lse, a_l, a_r)
+            ctx.graph, ctx.layer, ctx.heads = graph, layer, heads
+        return out
+
+    @staticmethod
+    def backward(ctx: Any, *grad_outputs: Tuple[Tensor, ...]):
+        z, z_halo, el, el_halo, er, out, lse, a_l, a_r = ctx.saved_tensors
+        grad = grad_outputs[0].contiguous()
+        heads, layer = ctx.heads, ctx.layer
+        n, F = z.shape
+        D = F // heads
+        s = (grad.view(n, heads, D) * out.view(n, heads, D)).sum(-1)
+        aux = torch.cat([er, lse, s], 1).contiguous()
+        g = ctx.graph.full if isinstance(ctx.graph, DecompGraph) else ctx.graph
+        dz = z.new_empty((n, F))
+        dl = z.new_empty((n, heads))
+        dr = z.new_empty((n, heads))
+        _, bwd_key = attn_keys(layer)
+
+        def aggregate(lo, hi, g_halo, aux_halo):
+            halo = (g_halo, z_halo, el_halo, aux_halo) if g_halo is not None else (None,) * 4
+            gat.backward(g, grad, halo[0], z, halo[1], el, halo[2], aux, halo[3], a_l, a_r, heads, lo, hi,
+                         dz[lo:hi], dl[lo:hi], dr[lo:hi])
+
+        quant = engine.ctx.bit_type == BitType.QUANT
+        _gat_propagate(f"backward{layer}", quant, grad, aux, bwd_key, True, aggregate)
+        zh = z.view(n, heads, D)
+        da_l = (dl.unsqueeze(-1) * zh).sum(0)
+        da_r = (dr.unsqueeze(-1) * zh).sum(0)
+        return dz, da_l.view_as(a_l), da_r.view_as(a_r), None, None, None, None

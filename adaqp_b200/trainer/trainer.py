@@ -17,7 +17,9 @@ from ..assigner import Assigner as assigner
 from ..communicator import Communicator as comm
 from ..helper import BitType, DistGNNType
 from ..manager import GraphEngine as engine
-from ..model import DistGCN, DistSAGE
+from ..communicator.p2p import gat_key_dims
+from ..model import DistGAT, DistGCN, DistSAGE
+from ..model.distGAT import gat_layer_shapes
 from .runtime_util import (aggregate_accuracy, aggregate_F1, setup_logger, sync_model, sync_seed,
                            train_for_one_epoch, val_test)
 
@@ -25,7 +27,9 @@ RUNING_MODE = ["Vanilla", "AdaQP", "AdaQP-q", "AdaQP-p"]
 # mode -> (message precision, overlap central aggregation with the exchange)
 QUNAT_PARA_MAP: Dict[str, Tuple[str, bool]] = {"Vanilla": ("full", False), "AdaQP": ("quant", True),
                                                "AdaQP-q": ("quant", False), "AdaQP-p": ("full", True)}
-MODEL_MAP: Dict[str, DistGNNType] = {"gcn": DistGNNType.DistGCN, "sage": DistGNNType.DistSAGE}
+# 'gat' is an extension beyond the reference's two models
+MODEL_MAP: Dict[str, DistGNNType] = {"gcn": DistGNNType.DistGCN, "sage": DistGNNType.DistSAGE, "gat": DistGNNType.DistGAT}
+GAT_HEADS = 4          # default of the yaml `model: gat_heads`
 
 
 class Trainer(object):
@@ -43,6 +47,8 @@ class Trainer(object):
         for k in ("assign_bits", "assign_cycle", "group_size", "coe_lambda"):
             if args.get(k) is not None:
                 self.config["assignment"][k] = args[k]
+        model = self.config["model"]
+        model["gat_heads"] = int(args["gat_heads"]) if args.get("gat_heads") is not None else int(model.get("gat_heads", GAT_HEADS))
         rt = self.config["runtime"]
         self.exp_path = f"{rt['exp_path']}/{dataset}/{rt['num_parts']}part/{rt['model_name']}"
         self.logger = setup_logger("trainer.log", rt["logger_level"], with_file=True)
@@ -70,6 +76,11 @@ class Trainer(object):
             raise ValueError(f"Invalid running mode: {rt['mode']}")
         if rt["model_name"] not in MODEL_MAP:
             raise ValueError(f"Invalid model type: {rt['model_name']}")
+        if MODEL_MAP[rt["model_name"]] == DistGNNType.DistGAT:
+            gat_layer_shapes(model["hidden_dim"], data["num_classes"], model["num_layers"], model["gat_heads"])
+            if comm.ctx.transport != "p2p":
+                raise NotImplementedError("model 'gat' runs on the p2p transport only; the CPU gloo plumbing mode "
+                                          "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports gcn and sage")
         precision, use_parallel = QUNAT_PARA_MAP[rt["mode"]]
         self.engine = engine(rt["num_epoches"], data["partition_path"], rt["dataset"], precision,
                              MODEL_MAP[rt["model_name"]], use_parallel)
@@ -82,14 +93,27 @@ class Trainer(object):
     def _set_buffer(self):
         data, model = self.config["data"], self.config["model"]
         shape = [data["num_feats"]] + [model["hidden_dim"]] * (model["num_layers"] - 1)
+        extra = {}
+        if self._is_gat():
+            # GAT exchanges the projected rows z of every layer (plus backward0 and the attention scalars)
+            shape, heads = self._gat_shapes()
+            extra["key_dims"] = gat_key_dims(shape, heads)
         comm.ctx.init_buffer(shape, engine.ctx.send_idx, engine.ctx.recv_idx, engine.ctx.bit_type,
-                             total_send_idx=engine.ctx.total_send_idx, num_remote=engine.ctx.num_remove)
+                             total_send_idx=engine.ctx.total_send_idx, num_remote=engine.ctx.num_remove, **extra)
+
+    def _is_gat(self) -> bool:
+        return MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistGAT
+
+    def _gat_shapes(self):
+        data, model = self.config["data"], self.config["model"]
+        return gat_layer_shapes(model["hidden_dim"], data["num_classes"], model["num_layers"], model["gat_heads"])
 
     def _set_assigner(self):
         data, model, rt, asg = (self.config[k] for k in ("data", "model", "runtime", "assignment"))
         self.assigner = assigner(data["num_feats"], model["hidden_dim"], model["num_layers"],
                                  asg["profile_data_length"], rt["assign_scheme"], asg["assign_bits"],
-                                 engine.ctx.scores, asg["group_size"], asg["coe_lambda"], asg["assign_cycle"])
+                                 engine.ctx.scores, asg["group_size"], asg["coe_lambda"], asg["assign_cycle"],
+                                 key_dims=gat_key_dims(*self._gat_shapes()) if self._is_gat() else None)
         self.logger.info(self.assigner)
 
     def _set_model(self):
@@ -99,6 +123,8 @@ class Trainer(object):
                   model["dropout_rate"], model["use_norm"])
         if kind == DistGNNType.DistGCN:
             self.model = DistGCN(*common).to(comm.ctx.device)
+        elif kind == DistGNNType.DistGAT:
+            self.model = DistGAT(*common, heads=model["gat_heads"]).to(comm.ctx.device)
         else:
             self.model = DistSAGE(*common, model["aggregator_type"]).to(comm.ctx.device)
 

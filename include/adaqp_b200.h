@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define ADAQP_ABI_VERSION 3
+#define ADAQP_ABI_VERSION 4
 
 #define ADAQP_EINVAL (-1)   /* bad argument (bits not in {1,2,4,8}, negative size ...) */
 #define ADAQP_EALIGN (-2)   /* pointer alignment requirement violated */
@@ -269,6 +269,35 @@ int adaqp_ln_relu_bwd_f32(const float *dy, int64_t lddy, const float *x, int64_t
 /* Row gather out[i] = x[idx[i]] (copy-buffer fills of ops.py:159-164; API parity only). */
 int adaqp_gather_rows_f32(const float *x, int64_t ld, const int64_t *idx, int64_t n,
                           int32_t F, float *out, int64_t ldo, void *stream);
+
+/* ------------------------------------------------------------ graph attention (GAT)
+ * DGL's GATConv aggregation (shared projection, negative slope 0.2, no attention dropout) over the halo exchange
+ * (csrc/gat.cu, host mirror adaqp_b200/gat.py); an extension beyond the reference, whose models are GCN and SAGE.
+ * Rows are F = H * D floats (H heads of width D); F <= 256, and when H > 1, D must be a multiple or a divisor of
+ * 32.  Per-head scalars are [rows, H] row-major.  As in adaqp_spmm_csr_seg_f32, source ids < n_split are local rows
+ * (z0, el0, ...) and ids >= n_split halo rows (z1, el1, ...; may be NULL when no row of the range has a halo
+ * neighbour); a launch covers destination rows [row_begin, row_end) and writes output row v at v - row_begin.
+ * No float atomics: equal inputs give bitwise equal outputs.
+ *
+ * scores: el[i,h] = <z[i,h,:], a_l[h,:]>, er[i,h] = <z[i,h,:], a_r[h,:]> for i < n_rows; a_l, a_r are [H * D]. */
+int adaqp_gat_scores_f32(const float *z, int64_t ldz, int64_t n_rows, int32_t H, int32_t F, const float *a_l,
+                         const float *a_r, float *el, float *er, void *stream);
+/* forward: e[v,u,h] = LeakyReLU(el[u,h] + er[v,h]) over the CSR row of v, lse[v,h] = logsumexp_u e[v,u,h],
+ * out[v,h,:] = sum_u exp(e[v,u,h] - lse[v,h]) z[u,h,:].  er covers the local rows (indexed by v). */
+int adaqp_gat_fwd_f32(const int64_t *indptr, const int32_t *indices, int64_t n_split, const float *z0, int64_t ldz0,
+                      const float *z1, int64_t ldz1, const float *el0, const float *el1, const float *er, int32_t H,
+                      int32_t F, int64_t row_begin, int64_t row_end, float *out, int64_t ldo, float *lse,
+                      void *stream);
+/* backward for local rows u (row_end <= n_split) of a symmetric graph, g = dL/dout, aux rows [er | lse | s] (3H
+ * floats, s[v,h] = <g[v,h,:], out[v,h,:]>):
+ *   t[v,u,h] = alpha[v,u,h] (<g[v,h,:], z[u,h,:]> - s[v,h]) (1 if el[u,h] + er[v,h] > 0 else 0.2)
+ *   del[u,h] = sum_{v in row u} t[v,u,h],  der[u,h] = sum_{w in row u} t[u,w,h]
+ *   dz[u] = sum_{v in row u} alpha[v,u] g[v] + del[u] a_l + der[u] a_r  (per head). */
+int adaqp_gat_bwd_f32(const int64_t *indptr, const int32_t *indices, int64_t n_split, const float *g0, int64_t ldg0,
+                      const float *g1, int64_t ldg1, const float *z0, int64_t ldz0, const float *z1, int64_t ldz1,
+                      const float *el0, const float *el1, const float *aux0, const float *aux1, const float *a_l,
+                      const float *a_r, int32_t H, int32_t F, int64_t row_begin, int64_t row_end, float *dz,
+                      int64_t lddz, float *del, float *der, void *stream);
 
 /* ------------------------------------------------------------ graph partitioning
  * Multilevel label-propagation k-way partitioning (csrc/partition.cu, level driver and host initial
