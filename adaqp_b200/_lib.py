@@ -20,7 +20,7 @@ i32 = C.c_int32
 u64 = C.c_uint64
 u32 = C.c_uint32
 
-ADAQP_ABI_VERSION = 4
+ADAQP_ABI_VERSION = 5
 MAX_PARTS = 64           # ADAQP_MAX_PARTS
 LP_HUB_DEGREE = 256      # ADAQP_LP_HUB_DEGREE
 IPC_HANDLE_BYTES = 64
@@ -112,6 +112,11 @@ SYMBOLS = {
     "adaqp_gat_bwd_f32": (C.c_int, [c_void_p, c_void_p, i64, c_void_p, i64, c_void_p, i64, c_void_p, i64, c_void_p, i64,
                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, i32, i32, i64, i64,
                                     c_void_p, i64, c_void_p, c_void_p, c_void_p]),
+    "adaqp_sage_pool_fwd_f32": (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, i64, c_void_p, i64, c_void_p, i64,
+                                          i32, i64, i64, C.c_int, c_void_p, i64, c_void_p, i64, c_void_p]),
+    "adaqp_sage_pool_bwd_f32": (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, i64, c_void_p, i64,
+                                          c_void_p, i64, c_void_p, i64, c_void_p, i64, i32, i64, i64, C.c_int,
+                                          c_void_p, i64, c_void_p]),
 }
 
 _lib = None

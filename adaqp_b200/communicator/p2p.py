@@ -66,8 +66,25 @@ def gat_key_dims(widths: Sequence[int], heads: Sequence[int]) -> Dict[str, int]:
     return dims
 
 
+def pool_arg_key(layer: int) -> str:
+    """fp32 key of the SAGE max-pool arg rows (int32 bit patterns), sent with the backward exchange of the layer."""
+    return f"pool_arg{layer}"
+
+
+def sage_pool_key_dims(widths: Sequence[int]) -> Dict[str, int]:
+    """Exchange keys and widths of a SAGE max-pool model whose layer l exchanges rows of p_l = relu(fc_pool(x_l))
+    (width widths[l], the layer's input width): test / forward / backward keys of every layer (backward0 included:
+    dW_pool of layer 0 needs the gradient of remote destinations), then the arg keys."""
+    L = len(widths)
+    dims = {f"test{i}": int(widths[i]) for i in range(L)}
+    dims.update({f"forward{i}": int(widths[i]) for i in range(L)})
+    dims.update({f"backward{i}": int(widths[i]) for i in range(L)})
+    dims.update({pool_arg_key(i): int(widths[i]) for i in range(L)})
+    return dims
+
+
 def quantisable(key: str) -> bool:
-    """Keys that may travel quantised (training exchanges of layer rows); test and attention keys are fp32."""
+    """Keys that may travel quantised (training exchanges of layer rows); test, attention and arg keys are fp32."""
     return key.startswith(("forward", "backward"))
 
 

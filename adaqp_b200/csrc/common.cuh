@@ -60,6 +60,13 @@ __device__ __forceinline__ void frontier_release(unsigned long long *counter) {
 }
 // The counter pair of (device, stream), allocated zeroed on first use (spmm.cu).
 unsigned long long *adaqp_frontier_counter(int dev, cudaStream_t s);
+// Grid of a one-warp-per-row frontier kernel: enough CTAs for every row, at most 8 per SM.
+inline int64_t adaqp_frontier_grid(int64_t rows, int warps_per_cta) {
+    const int sms = adaqp_sm_count() > 0 ? adaqp_sm_count() : 132;
+    int64_t grid = (rows + warps_per_cta - 1) / warps_per_cta;
+    if (grid > (int64_t)sms * 8) grid = (int64_t)sms * 8;
+    return grid;
+}
 
 // ---------------------------------------------------------------- Philox
 // Philox4x32-10 exactly as curand's curand_Philox4x32_10 (curand_philox4x32_x.h):

@@ -325,12 +325,7 @@ int head_layout(const char *what, int32_t H, int32_t F, int *mode, int *D, int *
     return 0;
 }
 
-int64_t frontier_grid(int64_t rows) {
-    const int sms = adaqp_sm_count() > 0 ? adaqp_sm_count() : 132;
-    int64_t grid = (rows + kWarps - 1) / kWarps;
-    if (grid > (int64_t)sms * 8) grid = (int64_t)sms * 8;
-    return grid;
-}
+int64_t frontier_grid(int64_t rows) { return adaqp_frontier_grid(rows, kWarps); }
 
 }  // namespace
 

@@ -17,9 +17,9 @@ import torch
 from torch import Tensor
 from torch.autograd import Function
 
-from .. import gat
+from .. import gat, sage_pool
 from ..communicator import Communicator as comm
-from ..communicator.p2p import attn_keys
+from ..communicator.p2p import attn_keys, pool_arg_key
 from ..helper import BitType, ProprogationMode
 from ..manager import DecompGraph
 from ..manager import GraphEngine as engine
@@ -263,19 +263,29 @@ def _gat_exchange(rows: Tensor, name: str, is_train: bool, scalars: Tensor, aux_
 def _gat_release(pend, aux_key: str):
     """After the last consumer of the received rows has been enqueued on the current stream."""
     pend.release()
-    comm.ctx.comm_buffer.p2p.release_fp(aux_key)
+    if aux_key is not None:
+        comm.ctx.comm_buffer.p2p.release_fp(aux_key)
 
 
-def _gat_propagate(name: str, quant: bool, rows: Tensor, scalars: Tensor, aux_key: str, is_train: bool, aggregate):
-    """Exchange + aggregation skeleton of full_graph_propagation / decomposed_graph_propagation for GAT:
-    aggregate(lo, hi, halo_rows, halo_scalars) runs the kernel over inner rows [lo, hi).  Central rows have no halo
-    neighbour in either direction, so in the overlapped mode they run while the exchange is in flight; the
-    marginal rows run in one pass once it has landed (their softmax spans local and halo sources)."""
+def _gat_propagate(name: str, quant: bool, rows: Tensor, scalars: Tensor, aux_key: str, is_train: bool, aggregate,
+                   split: bool = False):
+    """Exchange + aggregation skeleton of full_graph_propagation / decomposed_graph_propagation for the models with
+    their own kernels (GAT, SAGE max-pool): aggregate(lo, hi, halo_rows, halo_scalars) runs the kernel over inner
+    rows [lo, hi).  `scalars` (None: rows only) travel in fp32 on `aux_key`.  Central rows have no halo neighbour in
+    either direction, so in the overlapped mode they run while the exchange is in flight.  The marginal rows run in
+    one pass once it has landed, or, with `split` (a kernel whose local and halo sources combine exactly) and
+    ADAQP_MARGINAL_SPLIT on, as aggregate(..., part='local') in flight and aggregate(..., part='halo') after."""
     eng, timer = engine.ctx, engine.ctx.timer
     comm_name = f"{name}_quantization" if quant else f"{name}_communication"
+
+    def exchange(stream=None):
+        if scalars is None:
+            return halo_exchange(rows, name, is_train, stream=stream), None
+        return _gat_exchange(rows, name, is_train, scalars, aux_key, stream=stream)
+
     if not eng.use_parallel:
         with timer.record_events(comm_name):
-            pend, aux_halo = _gat_exchange(rows, name, is_train, scalars, aux_key)
+            pend, aux_halo = exchange()
         with timer.record_events(f"{name}_full_aggregation"):
             kept = aggregate(0, eng.num_inner, pend.halo, aux_halo)
         _gat_release(pend, aux_key)
@@ -285,21 +295,32 @@ def _gat_propagate(name: str, quant: bool, rows: Tensor, scalars: Tensor, aux_ke
     ready.record(main)                       # rows and scalars are produced on the default stream
     side.wait_event(ready)
     with timer.record_events(comm_name, stream=side):
-        pend, aux_halo = _gat_exchange(rows, name, is_train, scalars, aux_key, stream=side)
+        pend, aux_halo = exchange(stream=side)
     landed = torch.cuda.Event(enable_timing=True)
     landed.record(side)
     nc = eng.num_central
     with timer.record_events(f"{name}_central_aggregation"):
         aggregate(0, nc, None, None)
-    central_done = torch.cuda.Event(enable_timing=True)
-    central_done.record(main)
-    timer.record_exposed(name, central_done, landed)
-    main.wait_event(landed)
-    with timer.record_events(f"{name}_marginal_aggregation"):
-        kept = aggregate(nc, eng.num_inner, pend.halo, aux_halo)
+    if split and _split_marginal():
+        with timer.record_events(f"{name}_marginal_aggregation_local"):
+            aggregate(nc, eng.num_inner, None, None, part="local")
+        overlappable_done = torch.cuda.Event(enable_timing=True)
+        overlappable_done.record(main)
+        timer.record_exposed(name, overlappable_done, landed)
+        main.wait_event(landed)
+        with timer.record_events(f"{name}_marginal_aggregation_halo"):
+            kept = aggregate(nc, eng.num_inner, pend.halo, aux_halo, part="halo")
+    else:
+        central_done = torch.cuda.Event(enable_timing=True)
+        central_done.record(main)
+        timer.record_exposed(name, central_done, landed)
+        main.wait_event(landed)
+        with timer.record_events(f"{name}_marginal_aggregation"):
+            kept = aggregate(nc, eng.num_inner, pend.halo, aux_halo)
     _gat_release(pend, aux_key)
     rows.record_stream(side)
-    scalars.record_stream(side)
+    if scalars is not None:
+        scalars.record_stream(side)
     return kept
 
 
@@ -365,3 +386,55 @@ class DistAggGAT(Function):
         da_l = (dl.unsqueeze(-1) * zh).sum(0)
         da_r = (dr.unsqueeze(-1) * zh).sum(0)
         return dz, da_l.view_as(a_l), da_r.view_as(a_r), None, None, None, None
+
+
+# ---------------------------------------------------------------- SAGE max-pool
+class DistAggSAGEPool(Function):
+    """Max-pool aggregation of local + remote neighbours for GraphSAGE (DGL's aggregator_type='pool'; an extension
+    beyond the reference, whose aggregators are mean and gcn).
+
+    forward(p, graph, layer, is_train) -> m: the exchange moves the pooled rows p (key forward{l}, quantised per
+    mode; test{l} in evaluation) and sage_pool_fwd takes the column-wise max and its arg; the local / halo sources of
+    the marginal rows combine exactly, so they keep the two-pass overlap.  backward exchanges dL/dm (backward{l},
+    every layer) and the arg rows in fp32 (pool_arg{l}): the owner of a source cannot recompute the arg of a remote
+    destination, whose owner saw the dequantised copy of p.  sage_pool_bwd then routes the gradient to the arg
+    source through engine.ctx.pool_want.  p2p transport only.  The layer-0 evaluation cache never applies: the
+    exchanged rows are p, which depends on the weights."""
+
+    @staticmethod
+    def forward(ctx, p: Tensor, graph, layer: int, is_train: bool) -> Tensor:
+        if comm.ctx.transport != "p2p":
+            raise NotImplementedError("SAGE max-pool runs on the p2p transport only (not the CPU gloo plumbing mode)")
+        eng = engine.ctx
+        p = p.contiguous()
+        n, F = p.shape
+        g = graph.full if isinstance(graph, DecompGraph) else graph
+        m = p.new_empty((n, F))
+        arg = torch.empty((n, F), dtype=torch.int32, device=p.device)
+
+        def aggregate(lo, hi, p_halo, _, part=None):
+            sage_pool.forward(g, p, p_halo, lo, hi, m[lo:hi], arg[lo:hi], part=part)
+
+        quant = eng.bit_type == BitType.QUANT and is_train
+        _gat_propagate(f"forward{layer}", quant, p, None, None, is_train, aggregate, split=True)
+        if is_train:
+            ctx.save_for_backward(arg)
+            ctx.graph, ctx.layer = graph, layer
+        return m
+
+    @staticmethod
+    def backward(ctx: Any, *grad_outputs: Tuple[Tensor, ...]):
+        arg, = ctx.saved_tensors
+        grad = grad_outputs[0].contiguous()
+        g = ctx.graph.full if isinstance(ctx.graph, DecompGraph) else ctx.graph
+        want = engine.ctx.pool_want
+        dp = grad.new_empty(grad.shape)
+
+        def aggregate(lo, hi, g_halo, arg_halo, part=None):
+            a_halo = arg_halo.view(torch.int32) if arg_halo is not None else None
+            sage_pool.backward(g, want, grad, g_halo, arg, a_halo, lo, hi, dp[lo:hi], part=part)
+
+        quant = engine.ctx.bit_type == BitType.QUANT
+        _gat_propagate(f"backward{ctx.layer}", quant, grad, arg.view(torch.float32), pool_arg_key(ctx.layer), True,
+                       aggregate, split=True)
+        return dp, None, None, None

@@ -16,8 +16,10 @@ from torch import Tensor
 from ..assigner import Assigner as assigner
 from ..communicator import Communicator as comm
 from ..helper import BitType, DistGNNType
+from .. import sage_pool
+from ..manager import DecompGraph
 from ..manager import GraphEngine as engine
-from ..communicator.p2p import gat_key_dims
+from ..communicator.p2p import gat_key_dims, sage_pool_key_dims
 from ..model import DistGAT, DistGCN, DistSAGE
 from ..model.distGAT import gat_layer_shapes
 from .runtime_util import (aggregate_accuracy, aggregate_F1, setup_logger, sync_model, sync_seed,
@@ -49,6 +51,8 @@ class Trainer(object):
                 self.config["assignment"][k] = args[k]
         model = self.config["model"]
         model["gat_heads"] = int(args["gat_heads"]) if args.get("gat_heads") is not None else int(model.get("gat_heads", GAT_HEADS))
+        if args.get("aggregator_type") is not None:        # extension: run-time override of the yaml's aggregator
+            model["aggregator_type"] = args["aggregator_type"]
         rt = self.config["runtime"]
         self.exp_path = f"{rt['exp_path']}/{dataset}/{rt['num_parts']}part/{rt['model_name']}"
         self.logger = setup_logger("trainer.log", rt["logger_level"], with_file=True)
@@ -81,6 +85,9 @@ class Trainer(object):
             if comm.ctx.transport != "p2p":
                 raise NotImplementedError("model 'gat' runs on the p2p transport only; the CPU gloo plumbing mode "
                                           "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports gcn and sage")
+        if self._is_pool() and comm.ctx.transport != "p2p":
+            raise NotImplementedError("aggregator_type 'pool' runs on the p2p transport only; the CPU gloo plumbing mode "
+                                      "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports the mean and gcn aggregators")
         precision, use_parallel = QUNAT_PARA_MAP[rt["mode"]]
         self.engine = engine(rt["num_epoches"], data["partition_path"], rt["dataset"], precision,
                              MODEL_MAP[rt["model_name"]], use_parallel)
@@ -98,11 +105,38 @@ class Trainer(object):
             # GAT exchanges the projected rows z of every layer (plus backward0 and the attention scalars)
             shape, heads = self._gat_shapes()
             extra["key_dims"] = gat_key_dims(shape, heads)
+        elif self._is_pool():
+            # max-pool exchanges the pooled rows p of every layer (plus backward0 and the arg rows)
+            extra["key_dims"] = self._key_dims()
         comm.ctx.init_buffer(shape, engine.ctx.send_idx, engine.ctx.recv_idx, engine.ctx.bit_type,
                              total_send_idx=engine.ctx.total_send_idx, num_remote=engine.ctx.num_remove, **extra)
+        if self._is_pool():
+            self._set_pool_want()
+
+    def _set_pool_want(self):
+        """The backward match table of the max-pool aggregation, aligned with the CSR the kernels read; the peers'
+        recv_idx come from the exchange's set-up all-gather."""
+        eng, ex = engine.ctx, comm.ctx.comm_buffer.p2p
+        g = eng.graph.full if isinstance(eng.graph, DecompGraph) else eng.graph
+        want = sage_pool.pool_want(g.indptr.cpu().numpy(), g.indices.cpu().numpy(), g.n_inner, ex.recv_idx,
+                                   ex.send_idx, ex.total_send_idx, ex.peer_recv_idx)
+        eng.pool_want = torch.from_numpy(want).to(g.device)
 
     def _is_gat(self) -> bool:
         return MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistGAT
+
+    def _is_pool(self) -> bool:
+        return (MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistSAGE
+                and self.config["model"]["aggregator_type"] == "pool")
+
+    def _key_dims(self):
+        """Per-key exchange widths of the models with their own exchange protocol (None: the reference's keys)."""
+        if self._is_gat():
+            return gat_key_dims(*self._gat_shapes())
+        if self._is_pool():
+            data, model = self.config["data"], self.config["model"]
+            return sage_pool_key_dims([data["num_feats"]] + [model["hidden_dim"]] * (model["num_layers"] - 1))
+        return None
 
     def _gat_shapes(self):
         data, model = self.config["data"], self.config["model"]
@@ -113,7 +147,7 @@ class Trainer(object):
         self.assigner = assigner(data["num_feats"], model["hidden_dim"], model["num_layers"],
                                  asg["profile_data_length"], rt["assign_scheme"], asg["assign_bits"],
                                  engine.ctx.scores, asg["group_size"], asg["coe_lambda"], asg["assign_cycle"],
-                                 key_dims=gat_key_dims(*self._gat_shapes()) if self._is_gat() else None)
+                                 key_dims=self._key_dims())
         self.logger.info(self.assigner)
 
     def _set_model(self):

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define ADAQP_ABI_VERSION 4
+#define ADAQP_ABI_VERSION 5
 
 #define ADAQP_EINVAL (-1)   /* bad argument (bits not in {1,2,4,8}, negative size ...) */
 #define ADAQP_EALIGN (-2)   /* pointer alignment requirement violated */
@@ -298,6 +298,31 @@ int adaqp_gat_bwd_f32(const int64_t *indptr, const int32_t *indices, int64_t n_s
                       const float *el0, const float *el1, const float *aux0, const float *aux1, const float *a_l,
                       const float *a_r, int32_t H, int32_t F, int64_t row_begin, int64_t row_end, float *dz,
                       int64_t lddz, float *del, float *der, void *stream);
+
+/* ------------------------------------------------------------ GraphSAGE max-pool aggregation
+ * DGL's SAGEConv(aggregator_type='pool') neighbourhood max over the halo exchange (csrc/sage_pool.cu, host mirror
+ * adaqp_b200/sage_pool.py); an extension beyond the reference, whose aggregators are mean and gcn.  Rows are
+ * 0 < F <= 1024 floats.  As in adaqp_spmm_csr_seg_f32, source ids < n_split are local rows (x0, g0, a0) and ids
+ * >= n_split halo rows (x1, g1, a1; may be NULL when no visited entry is a halo source); seg_start / seg_end (NULL =
+ * the row bounds) restrict each row to [seg_start[v], seg_end[v]); a launch covers rows [row_begin, row_end) and
+ * writes row v at v - row_begin; accumulate != 0 continues from what the output already holds.  arg entries are
+ * (source id - n_split), INT32_MIN for a row without sources (whose m is 0).  No float atomics: equal inputs give
+ * bitwise equal outputs, and a local-segment launch followed by an accumulating halo-segment launch equals one
+ * launch over whole rows bit for bit.
+ *
+ * forward: m[v,c] = max_u x[u,c] over the row of v, arg[v,c] = the first u in CSR order attaining it. */
+int adaqp_sage_pool_fwd_f32(const int64_t *indptr, const int64_t *seg_start, const int64_t *seg_end,
+                            const int32_t *indices, int64_t n_split, const float *x0, int64_t ld0, const float *x1,
+                            int64_t ld1, int32_t F, int64_t row_begin, int64_t row_end, int accumulate, float *out,
+                            int64_t ldo, int32_t *arg, int64_t lda, void *stream);
+/* backward for local rows u (row_end <= n_split) of a symmetric graph, g = dL/dm, a = arg rows in their owner's
+ * encoding, want[e] (aligned with indices) = row u in the encoding of the owner of indices[e]:
+ *   dp[u,c] = sum_{e in row u} g[x_e,c] [a[x_e,c] == want[e]]   (sum in CSR order) */
+int adaqp_sage_pool_bwd_f32(const int64_t *indptr, const int64_t *seg_start, const int64_t *seg_end,
+                            const int32_t *indices, const int32_t *want, int64_t n_split, const float *g0,
+                            int64_t ldg0, const float *g1, int64_t ldg1, const int32_t *a0, int64_t lda0,
+                            const int32_t *a1, int64_t lda1, int32_t F, int64_t row_begin, int64_t row_end,
+                            int accumulate, float *dp, int64_t ldd, void *stream);
 
 /* ------------------------------------------------------------ graph partitioning
  * Multilevel label-propagation k-way partitioning (csrc/partition.cu, level driver and host initial

@@ -25,6 +25,8 @@ def parse():
     for flag, typ, default, text in FLAGS:
         p.add_argument(flag, type=typ, default=default, help=text)
     p.add_argument("--num_epoches", type=int, default=None, help="override the config's epoch count")
+    p.add_argument("--aggregator_type", type=str, default=None,
+                   help="GraphSAGE aggregator: mean, gcn or pool (default: the config's)")
     return p.parse_args()
 
 

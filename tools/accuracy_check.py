@@ -34,7 +34,8 @@ def run(mode, scheme, bits, seed, args, world):
     os.environ["ADAQP_SEED"] = str(seed)
     t = Trainer(Namespace(dataset=args.dataset, num_parts=world, backend="gloo", init_method="env://",
                           model_name=args.model_name, mode=mode, assign_scheme=scheme, logger_level="WARNING",
-                          num_epoches=args.epochs, exp_path="/tmp/adaqp_acc_exp", assign_bits=bits))
+                          num_epoches=args.epochs, exp_path="/tmp/adaqp_acc_exp", assign_bits=bits,
+                          aggregator_type=args.aggregator_type))
     if scheme == "adaptive":
         t.assigner.assign_cycle = args.assign_cycle
     t.train()
@@ -77,7 +78,8 @@ def worker(args):
         for r in runs:
             if r["name"] != "Vanilla":
                 delta.setdefault(r["name"], []).append(100 * (r["best_val"] - base[r["seed"]]))
-        summary = {"world": world, "epochs": args.epochs, "scale": args.scale, "model": args.model_name, "dataset": args.dataset,
+        summary = {"world": world, "epochs": args.epochs, "scale": args.scale, "model": args.model_name,
+                   "aggregator_type": args.aggregator_type, "dataset": args.dataset,
                    "feature_signal": signal, "label_noise": args.label_noise, "calibration": calib, "runs": runs,
                    "vanilla_best_val_mean": float(np.mean(list(base.values()))),
                    "delta_best_val_vs_vanilla_pp": {k: {"mean": float(np.mean(v)), "min": float(np.min(v)), "max": float(np.max(v)), "n": len(v)}
@@ -101,6 +103,7 @@ def main():
     ap.add_argument("--scale", type=float, default=0.05)
     ap.add_argument("--dataset", type=str, default="ogbn-products")
     ap.add_argument("--model_name", type=str, default="gcn")
+    ap.add_argument("--aggregator_type", type=str, default=None, help="GraphSAGE aggregator (default: the config's)")
     ap.add_argument("--assign_cycle", type=int, default=20)
     ap.add_argument("--seeds", type=int, default=3)
     ap.add_argument("--seed0", type=int, default=123)
