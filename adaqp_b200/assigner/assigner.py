@@ -15,6 +15,7 @@ import time
 from itertools import chain
 from typing import Dict, List, Tuple, Union
 
+import numpy as np
 import torch
 from torch import Tensor
 
@@ -67,6 +68,7 @@ class Assigner(object):
         self.traced_layer_data: Dict[str, Union[float, Tensor, Dict[int, Tensor]]] = {}
         self.group_idx: Dict[str, Dict[int, Tuple[Tensor, ...]]] = {}
         self.last_solve_seconds: Dict[str, float] = {}
+        self.assignment: Dict[str, Dict[int, Tensor]] = None     # the last get_assignment() result (checkpoints)
         if scheme == "adaptive" and engine.ctx.bit_type == BitType.QUANT:
             self._init_adaptive()
         Assigner.ctx = self
@@ -88,7 +90,41 @@ class Assigner(object):
     def get_assignment(self, send_idx: Dict[int, Tuple[int, int]], runtime_scheme: str = None):
         scheme = self._scheme if runtime_scheme is None else runtime_scheme
         assert scheme in ASSIGNMENT_SCHEME, f"assignment scheme {scheme} is not supported"
-        return self._scheme_map[scheme](send_idx)
+        self.assignment = self._scheme_map[scheme](send_idx)
+        return self.assignment
+
+    # ---- checkpoint state (trainer/checkpoint.py) -------------------------------------------------
+    def state_dict(self) -> dict:
+        """Everything a resumed run needs to draw the same assignments as a run that never stopped: the current
+        assignment, the traced variances accumulated since the last re-assignment (moved to the CPU), the fitted
+        cost model (timed, so a fresh process would fit a different one), `is_tracing` and `sample_rate`.  Plain
+        tensors, dicts and scalars only, so that `torch.load(..., weights_only=True)` reads it back."""
+        def traced(v):
+            return v.detach().cpu().clone() if isinstance(v, Tensor) else float(v)
+        return {"scheme": self._scheme,
+                "assignment": None if self.assignment is None else
+                {k: {int(p): torch.as_tensor(b, dtype=torch.int32).cpu().clone() for p, b in per.items()}
+                 for k, per in self.assignment.items()},
+                "traced_layer_data": {k: traced(v) for k, v in self.traced_layer_data.items()},
+                "cost_model": None if self.cost_model is None else
+                {k: torch.from_numpy(np.array(v, np.float64)) for k, v in self.cost_model.items()},
+                "is_tracing": bool(self.is_tracing),
+                "sample_rate": self.sample_rate.clone()}
+
+    def load_state_dict(self, state: dict, device: torch.device = None):
+        """Inverse of state_dict(); traced accumulators go to `device` (default: the communicator's device)."""
+        if state["scheme"] != self._scheme:
+            raise ValueError(f"assigner state of scheme {state['scheme']!r} cannot be loaded into scheme {self._scheme!r}")
+        if device is None:
+            device = comm.ctx.device if comm.ctx is not None else torch.device("cpu")
+        self.assignment = None if state["assignment"] is None else \
+            {k: {int(p): b.clone() for p, b in per.items()} for k, per in state["assignment"].items()}
+        self.traced_layer_data = {k: (v.to(device) if isinstance(v, Tensor) else float(v))
+                                  for k, v in state["traced_layer_data"].items()}
+        self.cost_model = None if state["cost_model"] is None else \
+            {k: v.numpy().copy() for k, v in state["cost_model"].items()}
+        self.is_tracing = bool(state["is_tracing"])
+        self.sample_rate = state["sample_rate"].clone()
 
     # ---- simple schemes (:95-120) ------------------------------------------------------------
     def _get_uniform_assignment(self, send_idx):

@@ -105,6 +105,8 @@ def save_rank_layout(layout: RankLayout, part_dir: str, dataset: str) -> str:
     os.makedirs(d, exist_ok=True)
     path = f"{d}/part{layout.rank}.npz"
     arrays = {k: np.ascontiguousarray(getattr(layout, k)) for k in _ARRAY_FIELDS}
+    if layout.inner_gid is not None:
+        arrays["inner_gid"] = np.ascontiguousarray(layout.inner_gid, np.int64)
     header = {k: (bool(getattr(layout, k)) if k == "is_bidirected" else int(getattr(layout, k))) for k in _SCALAR_FIELDS}
     header["send_idx"] = {str(p): [int(lo), int(hi)] for p, (lo, hi) in layout.send_idx.items()}
     header["recv_peers"] = [int(p) for p in layout.recv_idx]
@@ -127,6 +129,7 @@ def read_rank_layout(path: str) -> RankLayout:
     kw["send_idx"] = {int(p): (int(v[0]), int(v[1])) for p, v in h["send_idx"].items()}
     kw["recv_idx"] = {int(p): z[f"recv_idx_{int(p)}"] for p in h["recv_peers"]}
     kw["scores"] = {int(p): (z[f"score_fwd_{int(p)}"], z[f"score_bwd_{int(p)}"]) for p in h["score_peers"]}
+    kw["inner_gid"] = z["inner_gid"] if "inner_gid" in z.files else None      # optional: older files lack it
     return RankLayout(**kw)
 
 

@@ -12,7 +12,7 @@ from __future__ import annotations
 import json
 import os
 from dataclasses import dataclass
-from typing import Callable, Dict, List, Tuple
+from typing import Callable, Dict, List, Optional, Tuple
 
 import numpy as np
 import scipy.sparse as sp
@@ -46,12 +46,19 @@ class RankLayout:
     src_marginal_idx: np.ndarray
     src_central_idx: np.ndarray
     is_bidirected: bool = True
+    # int64 [n_inner], rows in [central | marginal] order: each inner node's id in the dataset's original
+    # numbering (what predictions are keyed by); None in files written before the field existed
+    inner_gid: Optional[np.ndarray] = None
 
 
 def _finish(raw: RawPartition, recv_idx, send_ids, scores) -> RankLayout:
     ro = cv.reorder_partition(raw, send_ids)
     send_idx, total = cv.convert_send_idx(ro.send_idx)
     sm, sc = cv.decomposition_indices(ro.indptr, ro.indices, ro.n_central, ro.n_inner)
+    inner_gid = None
+    if raw.inner_gid is not None:
+        inner_gid = np.empty(ro.n_inner, np.int64)
+        inner_gid[ro.new_id] = raw.inner_gid
     return RankLayout(rank=raw.rank, world_size=raw.num_parts, n_central=ro.n_central,
                       n_marginal=ro.n_marginal, n_inner=ro.n_inner, n_halo=ro.n_halo,
                       indptr=ro.indptr, indices=ro.indices, in_degrees=ro.in_degrees,
@@ -59,7 +66,7 @@ def _finish(raw: RawPartition, recv_idx, send_ids, scores) -> RankLayout:
                       train_mask=ro.train_mask, val_mask=ro.val_mask, test_mask=ro.test_mask,
                       send_idx=send_idx, total_send_idx=total, recv_idx=recv_idx, scores=scores,
                       src_marginal_idx=sm, src_central_idx=sc,
-                      is_bidirected=bool(np.array_equal(ro.in_degrees, ro.out_degrees)))
+                      is_bidirected=bool(np.array_equal(ro.in_degrees, ro.out_degrees)), inner_gid=inner_gid)
 
 
 def prepare_rank(spec: SynthSpec, rank: int, model_type: DistGNNType,
@@ -131,7 +138,8 @@ def raw_partitions(graph, part: np.ndarray) -> List[RawPartition]:
             indices=B.indices.astype(np.int32), halo_gid=halo_gid.astype(np.int64),
             halo_part=(np.searchsorted(starts, halo_gid, side="right") - 1).astype(np.int32),
             feat=graph.feat[ids], label=graph.label[ids], train_mask=graph.train_mask[ids],
-            val_mask=graph.val_mask[ids], test_mask=graph.test_mask[ids], in_degrees=d, out_degrees=d.copy()))
+            val_mask=graph.val_mask[ids], test_mask=graph.test_mask[ids], in_degrees=d, out_degrees=d.copy(),
+            inner_gid=ids.astype(np.int64)))
     return raws
 
 

@@ -99,6 +99,7 @@ class RawPartition:
     test_mask: np.ndarray
     in_degrees: Optional[np.ndarray] = None   # global degrees of all local nodes (inner + halo)
     out_degrees: Optional[np.ndarray] = None
+    inner_gid: Optional[np.ndarray] = None    # int64 [n_inner]: each inner node's id in the dataset's own numbering
 
     @property
     def n_halo(self) -> int:
@@ -252,7 +253,8 @@ def build_raw_partition(spec: SynthSpec, rank: int) -> RawPartition:
     return RawPartition(rank=rank, num_parts=W, n_inner=n, inner_start=g0, starts=starts,
                         indptr=A.indptr.astype(np.int64), indices=A.indices.astype(np.int32),
                         halo_gid=halo_gid.astype(np.int64), halo_part=halo_part, feat=feat,
-                        label=label, train_mask=tr, val_mask=va, test_mask=te)
+                        label=label, train_mask=tr, val_mask=va, test_mask=te,
+                        inner_gid=g0 + np.arange(n, dtype=np.int64))
 
 
 def attach_global_degrees(raw: RawPartition, inner_degrees_of_all: List[np.ndarray], starts: np.ndarray):

@@ -5,10 +5,12 @@ reference's main.py drives it unchanged."""
 from __future__ import annotations
 
 import csv
+import json
 import os
 from argparse import Namespace
 from typing import Dict, Tuple
 
+import numpy as np
 import torch
 import yaml
 from torch import Tensor
@@ -21,9 +23,11 @@ from ..manager import DecompGraph
 from ..manager import GraphEngine as engine
 from ..communicator.p2p import gat_key_dims, sage_pool_key_dims
 from ..model import DistGAT, DistGCN, DistSAGE
+from ..manager.graphEngine import load_rank_layout
 from ..model.distGAT import gat_layer_shapes
-from .runtime_util import (aggregate_accuracy, aggregate_F1, setup_logger, sync_model, sync_seed,
-                           train_for_one_epoch, val_test)
+from . import checkpoint as ckpt
+from .runtime_util import (_check_exchange_status, aggregate_accuracy, aggregate_F1, get_metrics, setup_logger,
+                           sync_model, sync_seed, train_for_one_epoch, val_test)
 
 RUNING_MODE = ["Vanilla", "AdaQP", "AdaQP-q", "AdaQP-p"]
 # mode -> (message precision, overlap central aggregation with the exchange)
@@ -54,6 +58,13 @@ class Trainer(object):
         if args.get("aggregator_type") is not None:        # extension: run-time override of the yaml's aggregator
             model["aggregator_type"] = args["aggregator_type"]
         rt = self.config["runtime"]
+        # extension: checkpoints (trainer/checkpoint.py); none of them set = no checkpoint files, as the reference
+        rt.setdefault("checkpoint_dir", None)
+        rt["checkpoint_every"] = int(rt.get("checkpoint_every") or 0)
+        rt.setdefault("resume", None)
+        if rt["checkpoint_every"] > 0 and not rt["checkpoint_dir"]:
+            raise ValueError("checkpoint_every > 0 needs checkpoint_dir")
+        self.resume_path, self.resume_epoch, self._partition_digest = None, 0, None
         self.exp_path = f"{rt['exp_path']}/{dataset}/{rt['num_parts']}part/{rt['model_name']}"
         self.logger = setup_logger("trainer.log", rt["logger_level"], with_file=True)
         self._set_communicator()
@@ -89,8 +100,16 @@ class Trainer(object):
             raise NotImplementedError("aggregator_type 'pool' runs on the p2p transport only; the CPU gloo plumbing mode "
                                       "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports the mean and gcn aggregators")
         precision, use_parallel = QUNAT_PARA_MAP[rt["mode"]]
+        layout = None
+        if rt["resume"]:
+            # a checkpoint that does not belong to this run is refused before any device work or exchange
+            layout = load_rank_layout(data["partition_path"], rt["dataset"], MODEL_MAP[rt["model_name"]])
+            self._partition_digest = ckpt.partition_digest(layout)
+            self.resume_path = ckpt.resolve(rt["resume"], rt["checkpoint_dir"])
+            self.resume_epoch = ckpt.check_resume(self.resume_path, self.run_fields(), self._partition_digest,
+                                                  rt["num_epoches"])
         self.engine = engine(rt["num_epoches"], data["partition_path"], rt["dataset"], precision,
-                             MODEL_MAP[rt["model_name"]], use_parallel)
+                             MODEL_MAP[rt["model_name"]], use_parallel, layout=layout)
         engine.ctx.agg_type = model["aggregator_type"]
         if engine.ctx.use_parallel:
             for g in (engine.ctx.graph, engine.ctx.bwd_graph):
@@ -142,6 +161,10 @@ class Trainer(object):
         data, model = self.config["data"], self.config["model"]
         return gat_layer_shapes(model["hidden_dim"], data["num_classes"], model["num_layers"], model["gat_heads"])
 
+    def run_fields(self) -> dict:
+        """What a checkpoint's manifest records about the run (trainer/checkpoint.py)."""
+        return ckpt.run_fields(self.config, self._key_dims())
+
     def _set_assigner(self):
         data, model, rt, asg = (self.config[k] for k in ("data", "model", "runtime", "assignment"))
         self.assigner = assigner(data["num_feats"], model["hidden_dim"], model["num_layers"],
@@ -166,10 +189,12 @@ class Trainer(object):
     def train(self):
         rt = self.config["runtime"]
         multilabel = self.config["data"]["is_multilabel"]
-        sync_seed()
-        self.model.reset_parameters()
-        sync_model(self.model)
+        if self.resume_path is None:
+            sync_seed()
+            self.model.reset_parameters()
+            sync_model(self.model)
         optimizer = torch.optim.Adam(self.model.parameters(), lr=rt["learning_rate"], weight_decay=rt["weight_decay"])
+        self.optimizer = optimizer
         criterion = torch.nn.BCEWithLogitsLoss(reduction="sum") if multilabel else torch.nn.CrossEntropyLoss(reduction="sum")
         eng = self.engine.ctx
         feats, labels = eng.feats, eng.labels
@@ -177,8 +202,18 @@ class Trainer(object):
         comm.all_reduce_sum(n_train)
         n_train = n_train.item()
         assign_time, train_time = [], []
-        self.exposed_comm_ms = []
-        for epoch in range(1, rt["num_epoches"] + 1):
+        self.exposed_comm_ms, self.losses = [], []
+        if self.resume_path is not None:
+            # in place of seeding and initialising: model, optimizer, RNG states, Assigner and Recorder of epoch E
+            rec = ckpt.load_run(self.resume_path, self.model, optimizer)
+            assign_time, train_time, self.exposed_comm_ms, self.losses = (
+                rec["assign_time"], rec["train_time"], rec["exposed_comm_ms"], rec["loss"])
+            self.logger.info(f"<resumed from {self.resume_path} at epoch {self.resume_epoch}>")
+        # per-epoch records of the whole run (resumed epochs included), as checkpoints carry them
+        self.epoch_records = {"assign_time": assign_time, "train_time": train_time,
+                              "exposed_comm_ms": self.exposed_comm_ms, "loss": self.losses}
+        best_val = float(eng.recorder.epoches_metrics[:self.resume_epoch, 1].max()) if self.resume_epoch else -float("inf")
+        for epoch in range(self.resume_epoch + 1, rt["num_epoches"] + 1):
             overhead, loss, traced, reduce_time = train_for_one_epoch(
                 epoch, eng.graph, self.model, feats, labels, optimizer, criterion, n_train, eng.train_mask)
             assign_time.append(overhead)
@@ -198,10 +233,86 @@ class Trainer(object):
                              f"{self.exposed_comm_ms[-1]:.3f}ms")
                     self.logger.info(info + "\n" + t)
                 comm.barrier()
+            self.losses.append(float(loss.detach()))
+            if rt["checkpoint_dir"]:
+                # outside the timed region of the epoch
+                row = eng.recorder.epoches_metrics[epoch - 1].tolist()
+                if row[1] > best_val:
+                    best_val = row[1]
+                    if comm.get_rank() == 0:
+                        ckpt.save_best(rt["checkpoint_dir"], epoch, self.model, self.run_fields(), row,
+                                       "f1_micro" if multilabel else "accuracy")
+                if rt["checkpoint_every"] > 0 and epoch % rt["checkpoint_every"] == 0:
+                    if self._partition_digest is None:
+                        self._partition_digest = ckpt.partition_digest(eng.layout)
+                    ckpt.save(rt["checkpoint_dir"], epoch, self.model, optimizer, self.run_fields(),
+                              self._partition_digest, self.epoch_records)
         tt = torch.tensor(train_time)
         records = torch.concat([torch.tensor(assign_time).sum().view(-1), tt.sum(dim=0)[0].view(-1), tt.mean(dim=0)])
         comm.ctx.delete_buffer()
         return records
+
+    # ---- inference ----------------------------------------------------------------------------------
+    def predict(self, checkpoint: str = None) -> Tensor:
+        """Load model weights from an epoch or `best` checkpoint (default `<checkpoint_dir>/best`; `auto` = the
+        latest epoch) and run one evaluation forward.  Returns this rank's [n_inner, C] logits in layout row order;
+        `predict_metrics` holds the global train / val / test metric.  The run may use another `num_parts` or
+        `mode` than the one that trained the weights."""
+        rt, eng = self.config["runtime"], self.engine.ctx
+        if checkpoint is None:
+            if not rt["checkpoint_dir"]:
+                raise ValueError("predict() needs a checkpoint directory or checkpoint_dir")
+            checkpoint = os.path.join(rt["checkpoint_dir"], "best")
+        path = ckpt.resolve(checkpoint, rt["checkpoint_dir"])
+        self.predict_manifest = ckpt.load_weights(path, self.model, self.run_fields())
+        self.predict_checkpoint = path
+        self.model.eval()
+        with torch.no_grad():
+            logits = self.model(eng.graph, eng.feats)
+        eng.timer.clear(is_train=False)
+        _check_exchange_status()
+        multilabel = self.config["data"]["is_multilabel"]
+        m = []
+        for mask in (eng.train_mask, eng.val_mask, eng.test_mask):
+            m.extend(float(x) for x in get_metrics(eng.labels[mask], logits[mask], multilabel))
+        m = torch.tensor(m, dtype=torch.float64)
+        comm.all_reduce_sum(m)
+        if multilabel:          # micro-F1 from the summed tp / predicted / actual counts, as aggregate_F1
+            self.predict_metrics = [float(2 * m[3 * k] / max(float(m[3 * k + 1] + m[3 * k + 2]), 1.0)) for k in range(3)]
+        else:
+            self.predict_metrics = [float(m[2 * k] / max(float(m[2 * k + 1]), 1.0)) for k in range(3)]
+        return logits
+
+    def save_predictions(self, out_dir: str, checkpoint: str = None) -> str:
+        """predict(), then each rank writes `out_dir/shard{r}.npz` (`node_id`, `logits`) and rank 0 merges the
+        shards from disk into `out_dir/predictions.npz`: `node_id` int64 [N] ascending, `logits` float32 [N, C]
+        and a JSON header with the checkpoint's epoch and the train / val / test metric."""
+        rank, W = comm.get_rank(), comm.get_world_size()
+        gid = engine.ctx.layout.inner_gid
+        if not all(comm.gather_all(gid is not None)):
+            raise ValueError("the partition files carry no original node ids (inner_gid): re-partition with "
+                             "graph_partition.py or tools/convert_dgl_partition.py to write predictions by node id")
+        logits = self.predict(checkpoint)
+        os.makedirs(out_dir, exist_ok=True)
+        np.savez(os.path.join(out_dir, f"shard{rank}.npz"), node_id=np.asarray(gid, np.int64),
+                 logits=logits.float().cpu().numpy())
+        comm.barrier()
+        final = os.path.join(out_dir, "predictions.npz")
+        if rank == 0:
+            shards = [np.load(os.path.join(out_dir, f"shard{r}.npz")) for r in range(W)]
+            ids = np.concatenate([s["node_id"] for s in shards])
+            order = np.argsort(ids, kind="stable")
+            header = {"checkpoint": self.predict_checkpoint, "epoch": int(self.predict_manifest["epoch"]),
+                      "num_parts": W, "metric": "f1_micro" if self.config["data"]["is_multilabel"] else "accuracy",
+                      **dict(zip(("train", "val", "test"), self.predict_metrics))}
+            tmp = os.path.join(out_dir, ".predictions.tmp.npz")
+            with open(tmp, "wb") as f:
+                np.savez(f, node_id=ids[order], logits=np.concatenate([s["logits"] for s in shards])[order],
+                         header_json=np.frombuffer(json.dumps(header).encode("utf-8"), dtype=np.uint8))
+            os.replace(tmp, final)
+        comm.barrier()
+        comm.ctx.delete_buffer()
+        return final
 
     def save(self, time_records: Tensor):
         if comm.get_rank() != 0:

@@ -27,9 +27,22 @@ def parse():
     p.add_argument("--num_epoches", type=int, default=None, help="override the config's epoch count")
     p.add_argument("--aggregator_type", type=str, default=None,
                    help="GraphSAGE aggregator: mean, gcn or pool (default: the config's)")
+    p.add_argument("--checkpoint_dir", type=str, default=None,
+                   help="directory for epoch checkpoints, `latest` and `best` (the best validation epoch's model)")
+    p.add_argument("--checkpoint_every", type=int, default=None, help="write a checkpoint every N epochs (0: off)")
+    p.add_argument("--resume", type=str, default=None,
+                   help="continue training from a checkpoint directory, or `auto` for <checkpoint_dir>/latest; "
+                        "with --predict_out: the checkpoint to predict from (default <checkpoint_dir>/best)")
+    p.add_argument("--predict_out", type=str, default=None,
+                   help="instead of training, write per-node predictions (logits by original node id) to this directory")
     return p.parse_args()
 
 
 if __name__ == "__main__":
-    trainer = Trainer(parse())
-    trainer.save(trainer.train())
+    args = parse()
+    if args.predict_out:
+        checkpoint, args.resume = args.resume, None          # weights only: no training state is resumed
+        Trainer(args).save_predictions(args.predict_out, checkpoint)
+    else:
+        trainer = Trainer(args)
+        trainer.save(trainer.train())

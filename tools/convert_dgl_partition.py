@@ -70,7 +70,9 @@ def raw_from_arrays(a: Dict[str, np.ndarray], rank: int, world: int):
         label=np.asarray(a["label"])[:n_in], train_mask=np.asarray(a["train_mask"], bool)[:n_in],
         val_mask=np.asarray(a["val_mask"], bool)[:n_in], test_mask=np.asarray(a["test_mask"], bool)[:n_in],
         in_degrees=np.asarray(a["in_degrees_global"])[orig].astype(np.int64),
-        out_degrees=np.asarray(a["out_degrees_global"])[orig].astype(np.int64))
+        out_degrees=np.asarray(a["out_degrees_global"])[orig].astype(np.int64),
+        # predictions are keyed by DGL's reshuffled global id (dgl.NID), the numbering the partition book uses
+        inner_gid=gid[:n_in].astype(np.int64))
 
 
 def convert(raws: List, model_type) -> List:
