@@ -154,7 +154,8 @@ def load():
 # environment variable -> library option (read ONCE, here; the library itself never reads the environment)
 ENV_OPTIONS = {"ADAQP_SPMM": "spmm_impl", "ADAQP_SPMM_GRAB": "spmm_rows_per_grab", "ADAQP_SPMM_CTAS": "spmm_ctas_per_sm",
                "ADAQP_SPMM_HINTS": "spmm_hints", "ADAQP_EXCH_SEND_CTAS": "exch_send_ctas",
-               "ADAQP_EXCH_RECV_CTAS": "exch_recv_ctas", "ADAQP_GEMM_BLOCK_K": "gemm_block_k"}
+               "ADAQP_EXCH_RECV_CTAS": "exch_recv_ctas", "ADAQP_GEMM_BLOCK_K": "gemm_block_k",
+               "ADAQP_SPMM_SLICE_COLS": "spmm_slice_cols"}
 
 
 def _apply_env_options(L):

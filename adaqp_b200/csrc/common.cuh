@@ -23,6 +23,7 @@ struct AdaqpOptions {
     int exch_send_ctas;       // 0 = one resident wave; > 0 = total CTA cap of the send kernels
     int exch_recv_ctas;       // same for the receive kernel
     int gemm_block_k;         // K block of gemm_tf32x3_kernel: 32 (SWIZZLE_128B, 2 stages) or 16 (SWIZZLE_64B, 4 stages)
+    int spmm_slice_cols;      // column-slice width of the default aggregation: 0 = automatic, >= F = unsliced
 };
 AdaqpOptions &adaqp_options();
 

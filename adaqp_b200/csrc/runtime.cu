@@ -25,7 +25,7 @@ int adaqp_check_launch(const char *what) {
 }
 
 AdaqpOptions &adaqp_options() {
-    static AdaqpOptions opt = {1, 0, 8, 0, 0, 0, 32};
+    static AdaqpOptions opt = {1, 0, 8, 0, 0, 0, 32, 0};
     return opt;
 }
 
@@ -40,6 +40,7 @@ int *option_slot(const char *name) {
     if (!strcmp(name, "exch_send_ctas")) return &o.exch_send_ctas;
     if (!strcmp(name, "exch_recv_ctas")) return &o.exch_recv_ctas;
     if (!strcmp(name, "gemm_block_k")) return &o.gemm_block_k;
+    if (!strcmp(name, "spmm_slice_cols")) return &o.spmm_slice_cols;
     return nullptr;
 }
 }  // namespace

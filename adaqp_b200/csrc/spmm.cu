@@ -174,6 +174,105 @@ spmm_csr_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ 
 }
 
 // ---------------------------------------------------------------------------------------
+// Column-sliced gather (the default path for 16-byte rows of 256, 384, ... columns, DESIGN §3).
+//
+// The F columns are aggregated as ceil(F / slice_cols) slices of at most slice_cols <= 128 columns in
+// one launch.  The frontier counter numbers the work (slice, row grab) slice-major, so every warp sweeps
+// slice 0 over all rows before slice 1 starts: the source rows a slice touches are slice_cols * 4 bytes
+// wide instead of F * 4, so the same L2 holds F / slice_cols times as many of the reused source rows.
+// One warp per destination row, one float4 column of the slice per lane, kUnroll neighbour rows in
+// flight per lane (the weights are shuffled after the loads are issued: 48 registers, no spills, the
+// same occupancy as spmm_csr_kernel<4, 2>).  Every output element is
+// the same __fmaf_rn chain in CSR order as spmm_csr_kernel's, followed by the same self term, mean,
+// post norm and accumulate, so the results are bitwise those of the unsliced kernel.
+__global__ void __launch_bounds__(kThreads)
+spmm_csr_sliced_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ indices,
+                       const float *__restrict__ x0, int64_t ld0, int64_t n_split,
+                       const float *__restrict__ x1, int64_t ld1,
+                       const float *__restrict__ pre, const float *__restrict__ post,
+                       int mean, int add_self, int64_t row_begin, int64_t row_end, int F, int slice_cols,
+                       float *__restrict__ out, int64_t ldo, unsigned long long *__restrict__ next_row, int rows_per_grab,
+                       const int64_t *__restrict__ seg_start, const int64_t *__restrict__ seg_end, int accumulate, int hints) {
+    const int lane = threadIdx.x & 31;
+    const int64_t n_rows = row_end - row_begin;
+    const int64_t n_grabs = (n_rows + rows_per_grab - 1) / rows_per_grab;
+    const int64_t n_units = n_grabs * ((F + slice_cols - 1) / slice_cols);
+    while (true) {
+        unsigned long long unit = 0;
+        if (lane == 0) unit = atomicAdd(next_row, 1ull);
+        unit = __shfl_sync(ADAQP_FULL_MASK, unit, 0);
+        if ((int64_t)unit >= n_units) break;
+        const int64_t slice = (int64_t)unit / n_grabs, grab = (int64_t)unit % n_grabs;
+        const int col = (int)slice * slice_cols + lane * 4;
+        const bool colok = lane * 4 < slice_cols && col < F;
+        const int64_t r_lo = row_begin + grab * rows_per_grab;
+        const int64_t r_hi = (r_lo + rows_per_grab < row_end) ? r_lo + rows_per_grab : row_end;
+        for (int64_t row = r_lo; row < r_hi; ++row) {
+            const int64_t row_b = __ldg(indptr + row), row_e = __ldg(indptr + row + 1);
+            const int64_t b = seg_start ? __ldg(seg_start + row) : row_b;
+            const int64_t e_ = seg_end ? __ldg(seg_end + row) : row_e;
+            float acc[4] = {0.f, 0.f, 0.f, 0.f};
+            for (int64_t j0 = b; j0 < e_; j0 += 32) {
+                const int n = (e_ - j0) < 32 ? (int)(e_ - j0) : 32;
+                int u = 0;
+                float w = 0.f;
+                if (lane < n) {
+                    u = (hints & kHintIndexStreaming) ? __ldcs(indices + j0 + lane) : __ldg(indices + j0 + lane);
+                    w = pre ? __ldg(pre + u) : 1.f;
+                }
+                for (int k = 0; k < n; k += kUnroll) {
+                    float v[kUnroll][4];
+#pragma unroll
+                    for (int t = 0; t < kUnroll; ++t) {
+                        const int uu = __shfl_sync(ADAQP_FULL_MASK, u, (k + t) & 31);
+                        const float *rs = (uu < n_split) ? (x0 + (int64_t)uu * ld0) : (x1 + ((int64_t)uu - n_split) * ld1);
+                        if ((k + t) < n && colok) {
+                            Vec<4>::load(rs + col, v[t]);
+                        } else {
+#pragma unroll
+                            for (int e = 0; e < 4; ++e) v[t][e] = 0.f;
+                        }
+                    }
+                    // the weights are shuffled once the loads are in flight: fewer live registers
+#pragma unroll
+                    for (int t = 0; t < kUnroll; ++t) {
+                        float wt = __shfl_sync(ADAQP_FULL_MASK, w, (k + t) & 31);
+                        if ((k + t) >= n) wt = 0.f;
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) acc[e] = __fmaf_rn(wt, v[t][e], acc[e]);
+                    }
+                }
+            }
+            if (!colok) continue;
+            if (add_self) {
+                const float ws = pre ? __ldg(pre + row) : 1.f;
+                const float *rs = (row < n_split) ? (x0 + row * ld0) : (x1 + (row - n_split) * ld1);
+                float v[4];
+                Vec<4>::load(rs + col, v);
+#pragma unroll
+                for (int e = 0; e < 4; ++e) acc[e] = __fmaf_rn(ws, v[e], acc[e]);
+            }
+            const float deg = (float)(row_e - row_b);       // mean divides by the full in-degree
+            const float ps = post ? __ldg(post + row) : 1.f;
+            float *orow = out + (row - row_begin) * ldo + col;
+            float prev[4];
+            if (accumulate) Vec<4>::load(orow, prev);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                float r = acc[e];
+                if (mean && deg > 0.f) r = __fdiv_rn(r, deg);
+                if (post) r = __fmul_rn(r, ps);
+                if (accumulate) r = __fadd_rn(prev[e], r);
+                acc[e] = r;
+            }
+            if (hints & kHintStoreStreaming) Vec<4>::store_cs(orow, acc);
+            else Vec<4>::store(orow, acc);
+        }
+    }
+    frontier_release(next_row);
+}
+
+// ---------------------------------------------------------------------------------------
 // v2: asynchronous row gather through a lane-private shared-memory ring (cp.async / LDGSTS).
 //
 // v1 stages gathered rows in registers: bytes in flight per SM are bounded by the register
@@ -566,6 +665,11 @@ spmm_csr_tma_kernel(const __grid_constant__ CUtensorMap map0, const __grid_const
 
 inline bool aligned(const void *p, int vec) { return ((uintptr_t)p & ((uintptr_t)vec * 4 - 1)) == 0; }
 
+// Slice width the default path picks for 16-byte rows when spmm_slice_cols is 0 (0 = unsliced): 128-column
+// slices when F is a multiple of 128 above 128, so every slice keeps all 32 lanes busy.  Slices with idle
+// lanes measured slower than the unsliced kernel (F = 200 as 2 x 100, F = 256 as 3 x 88 or 4 x 64; DESIGN §3).
+int auto_slice_cols(int F) { return (F > 128 && F % 128 == 0) ? 128 : 0; }
+
 }  // namespace
 
 namespace {
@@ -700,11 +804,32 @@ int adaqp_spmm_csr_seg_f32(const int64_t *indptr, const int64_t *seg_start, cons
         else { if (nchunks <= 1) launch(spmm_csr_tma_kernel<1, false>); else launch(spmm_csr_tma_kernel<2, false>); }
         return adaqp_check_launch("spmm_csr_tma_kernel");
     }
-    int64_t grid = (rows + kWarps - 1) / kWarps;
-    // 1 row per grab for wide rows, 2 for F <= 128 (option spmm_rows_per_grab overrides)
-    const int grab_now = opt.spmm_rows_per_grab > 0 ? opt.spmm_rows_per_grab : (F > 128 ? 1 : 2);
-    { const int64_t cap2 = (int64_t)sms * (opt.spmm_ctas_per_sm > 0 ? opt.spmm_ctas_per_sm : 8); if (grid > cap2) grid = cap2; }
+    const int64_t cta_cap = (int64_t)sms * (opt.spmm_ctas_per_sm > 0 ? opt.spmm_ctas_per_sm : 8);
     const int hints = opt.spmm_hints;
+    // column slices of 16-byte rows (spmm_csr_sliced_kernel); rows that are not 16-byte aligned stay unsliced
+    int slice = 0;
+    if (vec == 4) {
+        slice = opt.spmm_slice_cols > 0 ? opt.spmm_slice_cols : auto_slice_cols(F);
+        if (slice >= F) slice = 0;
+        ADAQP_REQUIRE(slice == 0 || (slice % 4 == 0 && slice <= 128), ADAQP_EINVAL,
+                      "adaqp_spmm_csr_seg_f32: slice width %d is not a multiple of 4 in [4, 128]", slice);
+    }
+    // one row per grab (option spmm_rows_per_grab overrides): the narrowest window of rows in flight, so most
+    // of the reused source rows stay in L2 (DESIGN §3: 1 row beat 2 by 4 % at F = 256 sliced, 3 % at F = 100)
+    const int grab_rows = opt.spmm_rows_per_grab > 0 ? opt.spmm_rows_per_grab : 1;
+    if (slice > 0) {
+        const int grab = grab_rows;
+        const int64_t units = ((rows + grab - 1) / grab) * ((F + slice - 1) / slice);
+        int64_t grid = (units + kWarps - 1) / kWarps;
+        if (grid > cta_cap) grid = cta_cap;
+        spmm_csr_sliced_kernel<<<(unsigned)grid, kThreads, 0, s>>>(indptr, indices, x0, ld0, n_split, x1, ld1, pre, post, mean,
+                                                                   add_self, row_begin, row_end, F, slice, out, ldo, counter, grab,
+                                                                   seg_start, seg_end, accumulate, hints);
+        return adaqp_check_launch("spmm_csr_sliced_kernel");
+    }
+    int64_t grid = (rows + kWarps - 1) / kWarps;
+    const int grab_now = grab_rows;
+    if (grid > cta_cap) grid = cta_cap;
 #define CALL_SPMM(V, C)                                                                           \
     spmm_csr_kernel<V, C><<<(unsigned)grid, kThreads, 0, s>>>(indptr, indices, x0, ld0, n_split, x1, \
                                                              ld1, pre, post, mean, add_self,      \
