@@ -11,7 +11,8 @@ the reference's host-side orchestration (paths relative to the reference tree, r
   mixed_dequantize   AdaQP/model/op_util.py:211-236
   exchange_*         AdaQP/model/op_util.py:137-187, AdaQP/communicator/comm.py:166-222
   gcn_aggregation    AdaQP/model/ops.py:17-32
-  sage_aggregation   AdaQP/model/ops.py:34-67
+  sage_aggregation   AdaQP/model/ops.py:34-67 (mean)
+  sage_gcn_aggregation  AdaQP/model/ops.py:34-67 (gcn)
   full/decomposed propagation   AdaQP/model/ops.py:132-193
 
 Parity pinning: see the header of quant_oracle.c (reference quant_cuda outputs
@@ -375,3 +376,18 @@ def sage_aggregation(indptr, indices, feats, in_deg, out_deg, n_dst: int, backwa
         return aggregate(indptr, indices, feats, mean=True)
     norm = _pow_clamped(out_deg, -1)
     return aggregate(indptr, indices, feats, pre=norm)
+
+
+def sage_gcn_aggregation(indptr, indices, feats, in_deg, out_deg, n_dst: int, backward: bool = False):
+    """ops.py:34-67, aggregator_type='gcn' (the neighbourhood includes the node itself):
+    forward  (sum_{u->v} x[u] + x[v]) / (clamp(in_deg[v], 1) + 1);
+    backward sum_{u->v} x[u] / (clamp(out_deg[u], 1) + 1) + x[v] / (clamp(out_deg[v], 1) + 1).
+    The norms are fp32 as in the reference (deg.float().clamp(min=1) + 1).pow(-1); the backward scales each
+    row by its norm in fp32 before the float64 sum, as `aggregate` does."""
+    x = _f32(feats)
+    if not backward:
+        post = _pow_clamped(np.maximum(np.asarray(in_deg, np.float32), np.float32(1.0)) + np.float32(1.0), -1)
+        out = aggregate(indptr, indices, x) + x[:n_dst].astype(np.float64)
+        return out * post[:n_dst, None].astype(np.float64)
+    pre = _pow_clamped(np.maximum(np.asarray(out_deg, np.float32), np.float32(1.0)) + np.float32(1.0), -1)
+    return aggregate(indptr, indices, x, pre=pre) + (x[:n_dst] * pre[:n_dst, None]).astype(np.float64)

@@ -47,10 +47,15 @@ def _oracle_forward(layouts, state, model_name, agg_type="mean"):
             if model_name == "gcn":
                 agg = O.gcn_aggregation(L.indptr, ix, full, L.in_degrees, L.out_degrees, L.n_inner)
                 y = agg @ state[f"convs.{l}.weight"].astype(np.float64) + state[f"convs.{l}.bias"]
-            else:
+            elif agg_type == "mean":
                 agg = O.sage_aggregation(L.indptr, ix, full, L.in_degrees, L.out_degrees, L.n_inner)
                 y = (h[r] @ state[f"sages.{l}.fc_self.weight"].astype(np.float64).T
                      + agg @ state[f"sages.{l}.fc_neigh.weight"].astype(np.float64).T + state[f"sages.{l}.bias"])
+            elif agg_type == "gcn":          # the self term is inside the aggregation; no fc_self
+                agg = O.sage_gcn_aggregation(L.indptr, ix, full, L.in_degrees, L.out_degrees, L.n_inner)
+                y = agg @ state[f"sages.{l}.fc_neigh.weight"].astype(np.float64).T + state[f"sages.{l}.bias"]
+            else:
+                raise ValueError(agg_type)
             if l < n_layers - 1:
                 mu = y.mean(1, keepdims=True)
                 var = y.var(1, keepdims=True)
@@ -95,7 +100,7 @@ def _worker(rank, world, port, tmp, mode, model_name, scheme, ngpu, out):
     err = 0.0
     if rank == 0:
         state = {k: v.detach().cpu().numpy() for k, v in tr.model.state_dict().items()}
-        want = _oracle_forward(layouts, state, model_name)[0]
+        want = _oracle_forward(layouts, state, model_name, eng.agg_type)[0]
         got = logits.cpu().numpy().astype(np.float64)
         err = float(np.abs(got - want).max() / (np.abs(want).max() + 1e-12))
     rec = tr.train()
