@@ -93,7 +93,7 @@ class CommBuffer(object):
 
     def get_train_buffer(self, layer: str):
         if self.bit_type == BitType.FULL:
-            return self.get_test_buffer(int(layer[-1]))
+            return self.get_test_buffer(p2p.layer_index(layer))
         return self.train_recv_buffers_cpu[layer], self.train_recv_buffers_gpu[layer], self.train_send_buffers_cpu[layer]
 
     def get_auxillary_buffer(self, layer: str):
@@ -130,7 +130,8 @@ class CommBuffer(object):
         rank, W = dist.get_rank(), dist.get_world_size()
         send_sizes: Dict[str, Dict[int, Dict[int, Tuple[int, int]]]] = {}
         for layer, per_peer in bits_assignment_rst.items():
-            dim = self.buffer_shape[int(layer[-1])]
+            # the key's real width (models with their own keys); the layer keys of buffer_shape otherwise
+            dim = self.p2p.dims[layer] if self.p2p is not None else self.buffer_shape[p2p.layer_index(layer)]
             self.send_original_idx_buffers[layer] = {}
             send_sizes[layer] = {}
             for pid, cfg in per_peer.items():

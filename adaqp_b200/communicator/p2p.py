@@ -17,6 +17,7 @@ buffer.py:32-34 "test" buffers).
 from __future__ import annotations
 
 import ctypes as C
+import re
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -42,8 +43,17 @@ def layer_keys(num_layers: int) -> List[str]:
     return keys
 
 
+def layer_index(key: str) -> int:
+    """Layer (or propagation step) index of a key: its whole trailing number ('forward10' -> 10).  The reference reads
+    the last character (buffer.py:63,201), which is the same for every key below 10."""
+    m = re.search(r"(\d+)$", key)
+    if m is None:
+        raise ValueError(f"exchange key {key!r} has no layer index")
+    return int(m.group(1))
+
+
 def key_dim(key: str, buffer_shape: Sequence[int]) -> int:
-    return int(buffer_shape[int(key[-1])])   # buffer.py:63,201: layer index = last character
+    return int(buffer_shape[layer_index(key)])
 
 
 def attn_keys(layer: int) -> Tuple[str, str]:
@@ -80,6 +90,17 @@ def sage_pool_key_dims(widths: Sequence[int]) -> Dict[str, int]:
     dims.update({f"forward{i}": int(widths[i]) for i in range(L)})
     dims.update({f"backward{i}": int(widths[i]) for i in range(L)})
     dims.update({pool_arg_key(i): int(widths[i]) for i in range(L)})
+    return dims
+
+
+def appnp_key_dims(num_classes: int, k: int) -> Dict[str, int]:
+    """Exchange keys of APPNP with K propagation steps: step k exchanges h_k on forward{k} (test{k} in evaluation)
+    and g_{k+1} on backward{k}; backward0 is needed because the MLP's weight gradients need g_0 at remote
+    destinations.  Every key is num_classes wide."""
+    C = int(num_classes)
+    dims = {f"test{i}": C for i in range(k)}
+    dims.update({f"forward{i}": C for i in range(k)})
+    dims.update({f"backward{i}": C for i in range(k)})
     return dims
 
 

@@ -61,6 +61,53 @@ template <> struct Vec<1> {
     static __device__ __forceinline__ void store_cs(float *p, const float (&v)[1]) { __stcs(p, v[0]); }
 };
 
+// One warp's weighted gather over the neighbour segment [b, e_) of a destination row:
+// acc += pre[u] * x[u] in CSR order, one __fmaf_rn per element and neighbour, the row's F floats spread
+// across lanes as VEC-wide vectors (CHUNKS per lane), neighbour ids fetched 32 at a time and broadcast by
+// shuffle, UNROLL_ neighbour rows (UNROLL_ * CHUNKS vector loads per lane) in flight.  Expanded in
+// spmm_csr_kernel and appnp_prop_kernel, so both sum in the same order.  A macro rather than an inlined
+// function: expanded in place, spmm_csr_kernel compiles to the same SASS as before appnp_prop_kernel
+// shared it (an inlined function changed its register allocation).  Reads acc, colok, lane, indices,
+// b, e_, x0, ld0, n_split, x1, ld1, pre and hints from the enclosing scope.
+#define ADAQP_GATHER_SEGMENT(UNROLL_) \
+        for (int64_t j0 = b; j0 < e_; j0 += 32) {                                                                       \
+            const int n = (e_ - j0) < 32 ? (int)(e_ - j0) : 32;                                                         \
+            int u = 0;                                                                                                  \
+            float w = 0.f;                                                                                              \
+            if (lane < n) {                                                                                             \
+                u = (hints & kHintIndexStreaming) ? __ldcs(indices + j0 + lane) : __ldg(indices + j0 + lane);           \
+                w = pre ? __ldg(pre + u) : 1.f;                                                                         \
+            }                                                                                                           \
+            for (int k = 0; k < n; k += UNROLL_) {                                                                      \
+                float v[UNROLL_][CHUNKS][VEC];                                                                          \
+                float ww[UNROLL_];                                                                                      \
+_Pragma("unroll")                                                                                                       \
+                for (int t = 0; t < UNROLL_; ++t) {                                                                     \
+                    const int src = (k + t) & 31;                                                                       \
+                    const int uu = __shfl_sync(ADAQP_FULL_MASK, u, src);                                                \
+                    ww[t] = __shfl_sync(ADAQP_FULL_MASK, w, src);                                                       \
+                    const bool live = (k + t) < n;                                                                      \
+                    if (!live) ww[t] = 0.f;                                                                             \
+                    const float *rp = (uu < n_split) ? (x0 + (int64_t)uu * ld0) : (x1 + ((int64_t)uu - n_split) * ld1); \
+_Pragma("unroll")                                                                                                       \
+                    for (int c = 0; c < CHUNKS; ++c) {                                                                  \
+                        if (live && colok[c]) {                                                                         \
+                            Vec<VEC>::load(rp + (c * 32 + lane) * VEC, v[t][c]);                                        \
+                        } else {                                                                                        \
+_Pragma("unroll")                                                                                                       \
+                            for (int e = 0; e < VEC; ++e) v[t][c][e] = 0.f;                                             \
+                        }                                                                                               \
+                    }                                                                                                   \
+                }                                                                                                       \
+_Pragma("unroll")                                                                                                       \
+                for (int t = 0; t < UNROLL_; ++t)                                                                       \
+_Pragma("unroll")                                                                                                       \
+                    for (int c = 0; c < CHUNKS; ++c)                                                                    \
+_Pragma("unroll")                                                                                                       \
+                        for (int e = 0; e < VEC; ++e) acc[c][e] = __fmaf_rn(ww[t], v[t][c][e], acc[c][e]);              \
+            }                                                                                                           \
+        }
+
 template <int VEC, int CHUNKS>
 __global__ void __launch_bounds__(kThreads)
 spmm_csr_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ indices,
@@ -98,43 +145,7 @@ spmm_csr_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ 
         const int64_t row_b = __ldg(indptr + row), row_e = __ldg(indptr + row + 1);
         const int64_t b = seg_start ? __ldg(seg_start + row) : row_b;
         const int64_t e_ = seg_end ? __ldg(seg_end + row) : row_e;
-        for (int64_t j0 = b; j0 < e_; j0 += 32) {
-            const int n = (e_ - j0) < 32 ? (int)(e_ - j0) : 32;
-            int u = 0;
-            float w = 0.f;
-            if (lane < n) {
-                u = (hints & kHintIndexStreaming) ? __ldcs(indices + j0 + lane) : __ldg(indices + j0 + lane);
-                w = pre ? __ldg(pre + u) : 1.f;
-            }
-            for (int k = 0; k < n; k += kUnroll) {
-                float v[kUnroll][CHUNKS][VEC];
-                float ww[kUnroll];
-#pragma unroll
-                for (int t = 0; t < kUnroll; ++t) {
-                    const int src = (k + t) & 31;
-                    const int uu = __shfl_sync(ADAQP_FULL_MASK, u, src);
-                    ww[t] = __shfl_sync(ADAQP_FULL_MASK, w, src);
-                    const bool live = (k + t) < n;
-                    if (!live) ww[t] = 0.f;
-                    const float *rp = (uu < n_split) ? (x0 + (int64_t)uu * ld0) : (x1 + ((int64_t)uu - n_split) * ld1);
-#pragma unroll
-                    for (int c = 0; c < CHUNKS; ++c) {
-                        if (live && colok[c]) {
-                            Vec<VEC>::load(rp + (c * 32 + lane) * VEC, v[t][c]);
-                        } else {
-#pragma unroll
-                            for (int e = 0; e < VEC; ++e) v[t][c][e] = 0.f;
-                        }
-                    }
-                }
-#pragma unroll
-                for (int t = 0; t < kUnroll; ++t)
-#pragma unroll
-                    for (int c = 0; c < CHUNKS; ++c)
-#pragma unroll
-                        for (int e = 0; e < VEC; ++e) acc[c][e] = __fmaf_rn(ww[t], v[t][c][e], acc[c][e]);
-            }
-        }
+        ADAQP_GATHER_SEGMENT(kUnroll)
         if (add_self) {
             const float ws = pre ? __ldg(pre + row) : 1.f;
             const float *rp = (row < n_split) ? (x0 + row * ld0) : (x1 + (row - n_split) * ld1);
@@ -169,6 +180,98 @@ spmm_csr_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ 
             }
         }
     }
+    }
+    frontier_release(next_row);
+}
+
+// ---------------------------------------------------------------------------------------
+// APPNP teleport propagation (DESIGN §13): spmm_csr_kernel's gather with the step's teleport term in the
+// epilogue, so a propagation step is one pass over [n, C] instead of an SpMM plus elementwise passes.
+//   r[v] = (scale * post[v]) * sum_{u in seg(v)} pre[u] x[u]
+//   EPI = kEpiTeleport: out[v] = r[v] + alpha * tele[v]                      (forward: tele = z)
+//   EPI = kEpiAccum   : out[v] = r[v];  a = alpha * x[v] (+ acc[v] with kAccRead)  (backward: x = g_{k+1})
+//                       acc[v] = a, or with kAccFold out[v] = r[v] + a and acc is only read (the last step writes dz)
+// The once-per-row terms (tele, acc) belong to the non-accumulating call of a row; an accumulating call
+// (the halo segment of a split row) adds only r[v] to what out holds.  The row's own operands (tele, acc and
+// x[v], or the accumulated output) are loaded before the gather, so their latency hides behind it instead of
+// following it (and acc[v] is written before the gather when it is not folded).  Rows of at most 4 floats per
+// lane are held to 40 registers, 6 CTAs = 48 warps per SM, the occupancy of spmm_csr_kernel at these widths.
+constexpr int kEpiTeleport = 0;
+constexpr int kEpiAccum = 1;
+constexpr int kAccRead = 2;    // acc_mode bits (bit 0: the acc term is on)
+constexpr int kAccFold = 4;
+
+template <int VEC, int CHUNKS, int EPI>
+__global__ void __launch_bounds__(kThreads, VEC * CHUNKS <= 2 ? 6 : (VEC * CHUNKS <= 4 ? 5 : 1))
+appnp_prop_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ indices,
+                  const float *__restrict__ x0, int64_t ld0, int64_t n_split,
+                  const float *__restrict__ x1, int64_t ld1,
+                  const float *__restrict__ pre, const float *__restrict__ post, float scale, float alpha,
+                  const float *__restrict__ tele, int64_t ldt, float *__restrict__ accv, int64_t lda, int acc_mode,
+                  int64_t row_begin, int64_t row_end, int F,
+                  float *__restrict__ out, int64_t ldo, unsigned long long *__restrict__ next_row,
+                  const int64_t *__restrict__ seg_start, const int64_t *__restrict__ seg_end, int accumulate) {
+    const int lane = threadIdx.x & 31;
+    bool colok[CHUNKS];
+#pragma unroll
+    for (int c = 0; c < CHUNKS; ++c) colok[c] = ((c * 32 + lane) * VEC) < F;
+    const int64_t n_rows = row_end - row_begin;
+    // what the epilogue adds to r: alpha * tele (teleport), a (folded acc term) or the accumulated output
+    const bool once = !accumulate;
+    const bool add_tele = EPI == kEpiTeleport && once && tele != nullptr;
+    const bool acc_on = EPI == kEpiAccum && once && (acc_mode & 1);
+    const bool fold = acc_on && (acc_mode & kAccFold);
+    while (true) {
+        unsigned long long grab = 0;
+        if (lane == 0) grab = atomicAdd(next_row, 1ull);       // one row per grab, as spmm_csr_kernel's default
+        grab = __shfl_sync(ADAQP_FULL_MASK, grab, 0);
+        if ((int64_t)grab >= n_rows) break;
+        const int64_t row = row_begin + (int64_t)grab;
+        const int64_t o = row - row_begin;
+        float *orow = out + o * ldo;
+        float addend[CHUNKS][VEC];
+#pragma unroll
+        for (int c = 0; c < CHUNKS; ++c) {
+            const int col = (c * 32 + lane) * VEC;
+#pragma unroll
+            for (int e = 0; e < VEC; ++e) addend[c][e] = 0.f;
+            if (!colok[c]) continue;
+            if (add_tele) {
+                Vec<VEC>::load(tele + o * ldt + col, addend[c]);
+            } else if (acc_on) {
+                float own[VEC];
+                Vec<VEC>::load(x0 + row * ld0 + col, own);
+                if (acc_mode & kAccRead) Vec<VEC>::load(accv + o * lda + col, addend[c]);
+#pragma unroll
+                for (int e = 0; e < VEC; ++e) addend[c][e] = __fmaf_rn(alpha, own[e], addend[c][e]);
+                if (!fold) Vec<VEC>::store(accv + o * lda + col, addend[c]);
+            } else if (accumulate) {
+                Vec<VEC>::load(orow + col, addend[c]);
+            }
+        }
+        float acc[CHUNKS][VEC];
+#pragma unroll
+        for (int c = 0; c < CHUNKS; ++c)
+#pragma unroll
+            for (int e = 0; e < VEC; ++e) acc[c][e] = 0.f;
+        const int64_t b = seg_start ? __ldg(seg_start + row) : __ldg(indptr + row);
+        const int64_t e_ = seg_end ? __ldg(seg_end + row) : __ldg(indptr + row + 1);
+        const int hints = 0;
+        ADAQP_GATHER_SEGMENT(kUnroll)
+        const float s = post ? __fmul_rn(scale, __ldg(post + row)) : scale;
+#pragma unroll
+        for (int c = 0; c < CHUNKS; ++c) {
+            if (!colok[c]) continue;
+            float r[VEC];
+#pragma unroll
+            for (int e = 0; e < VEC; ++e) {
+                r[e] = __fmul_rn(acc[c][e], s);
+                if (add_tele) r[e] = __fmaf_rn(alpha, addend[c][e], r[e]);
+                else if (fold) r[e] = __fadd_rn(r[e], addend[c][e]);
+                else if (accumulate) r[e] = __fadd_rn(addend[c][e], r[e]);
+            }
+            Vec<VEC>::store(orow + (c * 32 + lane) * VEC, r);
+        }
     }
     frontier_release(next_row);
 }
@@ -864,6 +967,75 @@ int adaqp_spmm_csr_f32(const int64_t *indptr, const int32_t *indices, const floa
                        int64_t row_end, int32_t F, float *out, int64_t ldo, void *stream) {
     return adaqp_spmm_csr_seg_f32(indptr, nullptr, nullptr, indices, x0, ld0, n_split, x1, ld1, pre, post, mean,
                                   add_self, 0, row_begin, row_end, F, out, ldo, stream);
+}
+
+int adaqp_appnp_prop_f32(const int64_t *indptr, const int64_t *seg_start, const int64_t *seg_end,
+                         const int32_t *indices, const float *x0, int64_t ld0, int64_t n_split, const float *x1,
+                         int64_t ld1, const float *pre, const float *post, float scale, float alpha,
+                         const float *tele, int64_t ldt, float *acc, int64_t lda, int32_t acc_mode, int accumulate,
+                         int64_t row_begin, int64_t row_end, int32_t F, float *out, int64_t ldo, void *stream) {
+    ADAQP_REQUIRE(F > 0 && F <= 1024, ADAQP_ELIMIT, "adaqp_appnp_prop_f32: F=%d outside (0,1024]", F);
+    ADAQP_REQUIRE(row_end >= row_begin && row_begin >= 0 && row_end <= n_split, ADAQP_EINVAL,
+                  "adaqp_appnp_prop_f32: bad row range [%lld, %lld) for n_split=%lld", (long long)row_begin,
+                  (long long)row_end, (long long)n_split);
+    ADAQP_REQUIRE(acc_mode >= 0 && acc_mode <= 7 && (acc_mode == 0 || (acc_mode & 1)), ADAQP_EINVAL,
+                  "adaqp_appnp_prop_f32: bad acc_mode %d", acc_mode);
+    ADAQP_REQUIRE(!(tele && acc_mode), ADAQP_EINVAL, "adaqp_appnp_prop_f32: tele and acc_mode are exclusive");
+    if (row_end == row_begin) return 0;
+    ADAQP_REQUIRE(indptr && indices && x0 && out, ADAQP_EINVAL, "adaqp_appnp_prop_f32: null pointer");
+    const bool need_acc = (acc_mode & kAccRead) || (acc_mode && !(acc_mode & kAccFold));
+    ADAQP_REQUIRE(!need_acc || acc, ADAQP_EINVAL, "adaqp_appnp_prop_f32: null acc for acc_mode %d", acc_mode);
+    // halo rows arrive as the exchange leaves them ([num_remote, F] contiguous): 4-byte aligned for odd F
+    int vec = 4;
+    auto fits = [&](int v) {
+        if (F % v || ld0 % v || ldo % v) return false;
+        if (!aligned(x0, v) || !aligned(out, v)) return false;
+        if (x1 && (!aligned(x1, v) || (ld1 % v))) return false;
+        if (tele && (!aligned(tele, v) || (ldt % v))) return false;
+        if (acc && (!aligned(acc, v) || (lda % v))) return false;
+        return true;
+    };
+    while (vec > 1 && !fits(vec)) vec >>= 1;
+    const int nchunks = (F + 32 * vec - 1) / (32 * vec);
+    int dev = 0;
+    ADAQP_CUDA(cudaGetDevice(&dev));
+    cudaStream_t s = (cudaStream_t)stream;
+    unsigned long long *counter = frontier_counter(dev, s);
+    ADAQP_REQUIRE(counter != nullptr, ADAQP_EINVAL, "adaqp_appnp_prop_f32: row counter allocation failed");
+    const int64_t grid = adaqp_frontier_grid(row_end - row_begin, kWarps);
+    const bool fwd = tele != nullptr || acc_mode == 0;
+    auto launch = [&](auto kernel) {
+        kernel<<<(unsigned)grid, kThreads, 0, s>>>(indptr, indices, x0, ld0, n_split, x1, ld1, pre, post, scale, alpha,
+                                                   tele, ldt, acc, lda, acc_mode, row_begin, row_end, F, out, ldo,
+                                                   counter, seg_start, seg_end, accumulate);
+    };
+#define APPNP_PICK(V, C)                                                                                    \
+    do {                                                                                                    \
+        if (fwd) launch(appnp_prop_kernel<V, C, kEpiTeleport>);                                             \
+        else launch(appnp_prop_kernel<V, C, kEpiAccum>);                                                    \
+    } while (0)
+    // the narrowest instantiation that holds the row: C = 47 is <1, 2>, C = 100 <4, 1>, C = 107 <1, 4>
+    if (vec == 4) {
+        if (nchunks <= 1) APPNP_PICK(4, 1);
+        else if (nchunks <= 2) APPNP_PICK(4, 2);
+        else if (nchunks <= 4) APPNP_PICK(4, 4);
+        else APPNP_PICK(4, 8);
+    } else if (vec == 2) {
+        if (nchunks <= 1) APPNP_PICK(2, 1);
+        else if (nchunks <= 2) APPNP_PICK(2, 2);
+        else if (nchunks <= 4) APPNP_PICK(2, 4);
+        else if (nchunks <= 8) APPNP_PICK(2, 8);
+        else APPNP_PICK(2, 16);
+    } else {
+        if (nchunks <= 1) APPNP_PICK(1, 1);
+        else if (nchunks <= 2) APPNP_PICK(1, 2);
+        else if (nchunks <= 4) APPNP_PICK(1, 4);
+        else if (nchunks <= 8) APPNP_PICK(1, 8);
+        else if (nchunks <= 16) APPNP_PICK(1, 16);
+        else APPNP_PICK(1, 32);
+    }
+#undef APPNP_PICK
+    return adaqp_check_launch("appnp_prop_kernel");
 }
 
 }  // extern "C"

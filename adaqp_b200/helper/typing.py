@@ -10,6 +10,7 @@ class DistGNNType(enum.Enum):
     DistGCN = 0
     DistSAGE = 1
     DistGAT = 2     # extension beyond the reference
+    DistAPPNP = 3   # extension beyond the reference
 
 
 @enum.unique

@@ -85,3 +85,49 @@ def spmm(graph: LocalGraph, x_local: torch.Tensor, x_halo: Optional[torch.Tensor
         out.stride(0), _lib.stream_ptr(stream))
     _lib.check(rc, "adaqp_spmm_csr_seg_f32")
     return out
+
+
+# acc_mode bits of appnp_prop (include/adaqp_b200.h): the acc term is on / continue from acc / fold it into out
+ACC_ON, ACC_READ, ACC_FOLD = 1, 2, 4
+
+
+def appnp_prop(graph: LocalGraph, x_local: torch.Tensor, x_halo: Optional[torch.Tensor],
+               pre: Optional[torch.Tensor], post: Optional[torch.Tensor], scale: float, alpha: float,
+               row_begin: int = 0, row_end: Optional[int] = None, out: Optional[torch.Tensor] = None,
+               tele: Optional[torch.Tensor] = None, acc: Optional[torch.Tensor] = None, acc_mode: int = 0,
+               stream=None, part: Optional[str] = None) -> torch.Tensor:
+    """One APPNP propagation step over CSR rows [row_begin, row_end) (csrc/spmm.cu appnp_prop_kernel):
+        out[v - row_begin] = scale * post[v] * sum_u pre[u] x[u]  (+ alpha * tele[v - row_begin])
+    and, with acc_mode (backward), acc[v - row_begin] = alpha * x[v] (+ acc[..] with ACC_READ), or with ACC_FOLD
+    the acc term added to out instead.  `tele`, `acc` and `out` are indexed like out.  part='local' / 'halo' as in
+    spmm(): the halo part accumulates its segment's share into `out` and adds no tele / acc term."""
+    L = _lib.load()
+    row_end = graph.n_inner if row_end is None else int(row_end)
+    F = int(x_local.shape[1])
+    assert x_local.dtype == torch.float32 and x_local.stride(1) == 1
+    if out is None:
+        out = torch.empty((row_end - row_begin, F), dtype=torch.float32, device=x_local.device)
+    if x_halo is not None and x_halo.shape[0] == 0:
+        x_halo = None
+    seg_start = seg_end = None
+    accumulate = 0
+    if part == "local":
+        seg_end = graph.halo_split.data_ptr()
+    elif part == "halo":
+        seg_start = graph.halo_split.data_ptr()
+        accumulate = 1
+    elif part is not None:
+        raise ValueError(part)
+    for t in (tele, acc):
+        assert t is None or (t.dtype == torch.float32 and t.stride(1) == 1 and t.shape[0] >= row_end - row_begin)
+    rc = L.adaqp_appnp_prop_f32(
+        graph.indptr.data_ptr(), seg_start, seg_end, graph.indices.data_ptr(), x_local.data_ptr(), x_local.stride(0),
+        graph.n_inner, x_halo.data_ptr() if x_halo is not None else None,
+        x_halo.stride(0) if x_halo is not None else 0,
+        pre.data_ptr() if pre is not None else None, post.data_ptr() if post is not None else None,
+        float(scale), float(alpha), tele.data_ptr() if tele is not None else None,
+        tele.stride(0) if tele is not None else 0, acc.data_ptr() if acc is not None else None,
+        acc.stride(0) if acc is not None else 0, int(acc_mode), accumulate, int(row_begin), row_end, F,
+        out.data_ptr(), out.stride(0), _lib.stream_ptr(stream))
+    _lib.check(rc, "adaqp_appnp_prop_f32")
+    return out

@@ -21,6 +21,7 @@ from .. import quant as integer_quantizer
 from ..assigner import Assigner as assigner
 from ..communicator import Basic_Buffer_Type
 from ..communicator import Communicator as comm
+from ..communicator.p2p import layer_index
 from ..helper import BitType
 from ..manager import GraphEngine as engine
 
@@ -91,7 +92,7 @@ def halo_exchange(messages: Tensor, name: str, is_train: bool, gathered: bool = 
     `messages` is the local message matrix [num_inner, F], or send_messages when gathered."""
     ex = comm.ctx.comm_buffer.p2p
     quant = engine.ctx.bit_type == BitType.QUANT and is_train
-    key = name if is_train else f"test{int(name[-1])}"
+    key = name if is_train else f"test{layer_index(name)}"
     if not quant:
         if assigner.ctx is not None and assigner.ctx.is_tracing:   # eval passes are traced too (op_util.py:91-99)
             _trace_rows(messages, name, gathered)
@@ -140,7 +141,7 @@ def msg_all2all_GLOO(send_messages: Tensor, name: str, is_train: bool = True) ->
 def fp_msg_transfer_process(send_messages, send_idx, recv_idx: Basic_Buffer_Type, msg_dim, msg_dtype,
                             num_remote, name, is_train) -> Tensor:
     buf = comm.ctx.comm_buffer
-    recv_cpu, recv_gpu, send_cpu = buf.get_train_buffer(name) if is_train else buf.get_test_buffer(int(name[-1]))
+    recv_cpu, recv_gpu, send_cpu = buf.get_train_buffer(name) if is_train else buf.get_test_buffer(layer_index(name))
     with engine.ctx.timer.record(f"{name}_communication"):
         comm.ctx.fp_msg_exchange(recv_cpu, recv_gpu, send_cpu, send_idx, send_messages)
     remote = torch.zeros(num_remote, msg_dim, dtype=msg_dtype, device=comm.ctx.device)

@@ -23,7 +23,7 @@ from ..communicator.p2p import attn_keys, pool_arg_key
 from ..helper import BitType, ProprogationMode
 from ..manager import DecompGraph
 from ..manager import GraphEngine as engine
-from ..manager.graph import LocalGraph, spmm
+from ..manager.graph import ACC_FOLD, ACC_ON, ACC_READ, LocalGraph, appnp_prop, spmm
 from ..manager.graphEngine import RowRange
 from .op_util import halo_exchange, msg_all2all_GLOO
 
@@ -438,3 +438,60 @@ class DistAggSAGEPool(Function):
         _gat_propagate(f"backward{ctx.layer}", quant, grad, arg.view(torch.float32), pool_arg_key(ctx.layer), True,
                        aggregate, split=True)
         return dp, None, None, None
+
+
+# ---------------------------------------------------------------- APPNP
+class DistAPPNPProp(Function):
+    """K personalized-PageRank steps of APPNP over the halo exchange (an extension beyond the reference):
+
+        h_0 = z,   h_{k+1} = (1 - alpha) A h_k + alpha z,   returns h_K      A = D^-1/2 A D^-1/2 (the GCN norms)
+
+    Step k exchanges h_k on forward{k} (quantised per mode; test{k} in evaluation) and runs appnp_prop_kernel, whose
+    epilogue adds the teleport term alpha z.  The propagation is linear in z, so backward saves nothing:
+    g_k = (1 - alpha) A^T g_{k+1} exchanges g_{k+1} on backward{k} (k = K-1 .. 0), the kernel also accumulates
+    alpha g_{k+1} of each row, and the last step writes dz = alpha sum_{k=1..K} g_k + g_0 directly.  Quantisation is
+    the identity in backward (straight-through), as in DistAggConv.  Every step keeps the overlap of
+    _gat_propagate with the two-pass marginal rows.  p2p transport only; the layer-0 evaluation cache does not apply
+    (z depends on the weights)."""
+
+    @staticmethod
+    def forward(ctx, z: Tensor, graph, k: int, alpha: float, is_train: bool) -> Tensor:
+        if comm.ctx.transport != "p2p":
+            raise NotImplementedError("APPNP runs on the p2p transport only (not the CPU gloo plumbing mode)")
+        eng = engine.ctx
+        z = z.contiguous()
+        g = graph.full if isinstance(graph, DecompGraph) else graph
+        pre, post = g.norm["out_-0.5"], g.norm["in_-0.5"]
+        quant = eng.bit_type == BitType.QUANT and is_train
+        h = z
+        for step in range(k):
+            out = torch.empty_like(z)
+
+            def aggregate(lo, hi, h_halo, _, part=None, h=h, out=out):
+                appnp_prop(g, h, h_halo, pre, post, 1.0 - alpha, alpha, lo, hi, out[lo:hi], tele=z[lo:hi], part=part)
+
+            _gat_propagate(f"forward{step}", quant, h, None, None, is_train, aggregate, split=True)
+            h = out
+        ctx.graph, ctx.k, ctx.alpha = graph, k, alpha
+        return h
+
+    @staticmethod
+    def backward(ctx: Any, *grad_outputs: Tuple[Tensor, ...]):
+        grad = grad_outputs[0].contiguous()
+        k, alpha = ctx.k, ctx.alpha
+        g = ctx.graph.full if isinstance(ctx.graph, DecompGraph) else ctx.graph
+        pre, post = g.norm["in_-0.5"], g.norm["out_-0.5"]
+        quant = engine.ctx.bit_type == BitType.QUANT
+        acc = torch.empty_like(grad)             # alpha * sum of the g_{k+1} seen so far
+        nxt = grad                               # g_{k+1}
+        for step in range(k - 1, -1, -1):
+            out = torch.empty_like(grad)
+            mode = ACC_ON | (ACC_READ if step < k - 1 else 0) | (ACC_FOLD if step == 0 else 0)
+
+            def aggregate(lo, hi, g_halo, _, part=None, nxt=nxt, out=out, mode=mode):
+                appnp_prop(g, nxt, g_halo, pre, post, 1.0 - alpha, alpha, lo, hi, out[lo:hi], acc=acc[lo:hi],
+                           acc_mode=mode, part=part)
+
+            _gat_propagate(f"backward{step}", quant, nxt, None, None, True, aggregate, split=True)
+            nxt = out
+        return nxt, None, None, None, None

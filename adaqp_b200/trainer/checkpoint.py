@@ -31,6 +31,9 @@ FORMAT_VERSION = 1
 RUN_FIELDS = ("dataset", "model_name", "aggregator_type", "gat_heads", "layer_dims", "num_parts", "mode",
               "assign_scheme", "key_dims")
 MODEL_FIELDS = RUN_FIELDS[:5]
+# fields added after format 1 was fixed, compared on resume and on prediction: a manifest written before a field
+# existed reads as null, which is what runs of the models without it record.  `propagation` is APPNP's {k, alpha}.
+ADDED_FIELDS = ("propagation",)
 
 
 # ----------------------------------------------------------------------------- descriptions of the run
@@ -44,7 +47,9 @@ def run_fields(config: dict, key_dims: Optional[Dict[str, int]]) -> dict:
     return {"dataset": rt["dataset"], "model_name": rt["model_name"], "aggregator_type": model["aggregator_type"],
             "gat_heads": int(model["gat_heads"]), "layer_dims": [int(data["num_feats"])] + [H] * (L - 1) + [int(data["num_classes"])],
             "num_parts": int(rt["num_parts"]), "mode": rt["mode"], "assign_scheme": rt["assign_scheme"],
-            "key_dims": {k: int(v) for k, v in key_dims.items()}}
+            "key_dims": {k: int(v) for k, v in key_dims.items()},
+            "propagation": ({"k": int(model["appnp_k"]), "alpha": float(model["appnp_alpha"])}
+                            if rt["model_name"] == "appnp" else None)}
 
 
 def partition_digest(layout) -> dict:
@@ -96,7 +101,7 @@ def resume_error(path: str, fields: dict, digest: dict, rank: int, num_epoches: 
         manifest = read_manifest(path)
     except FileNotFoundError as e:
         return e
-    err = _compare(manifest, fields, RUN_FIELDS)
+    err = _compare(manifest, fields, RUN_FIELDS + ADDED_FIELDS)
     if err is not None:
         return err
     for r in range(fields["num_parts"]):
@@ -265,7 +270,7 @@ def load_weights(path: str, model, fields: dict) -> dict:
     """Model weights only (epoch or best checkpoint), for prediction: the model fields must match; the partition,
     `num_parts` and `mode` may differ, since weights do not depend on them.  Returns the manifest."""
     manifest = read_manifest(path)
-    err = _compare(manifest, fields, MODEL_FIELDS)
+    err = _compare(manifest, fields, MODEL_FIELDS + ADDED_FIELDS)
     if err is not None:
         raise err
     model.load_state_dict(_load(os.path.join(path, "model.pt"))["model"])

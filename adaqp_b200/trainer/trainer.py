@@ -21,8 +21,9 @@ from ..helper import BitType, DistGNNType
 from .. import sage_pool
 from ..manager import DecompGraph
 from ..manager import GraphEngine as engine
-from ..communicator.p2p import gat_key_dims, sage_pool_key_dims
-from ..model import DistGAT, DistGCN, DistSAGE
+from ..communicator.p2p import appnp_key_dims, gat_key_dims, sage_pool_key_dims
+from ..model import DistAPPNP, DistGAT, DistGCN, DistSAGE
+from ..model.distAPPNP import APPNP_ALPHA, APPNP_K, appnp_params
 from ..manager.graphEngine import load_rank_layout
 from ..model.distGAT import gat_layer_shapes
 from . import checkpoint as ckpt
@@ -33,8 +34,9 @@ RUNING_MODE = ["Vanilla", "AdaQP", "AdaQP-q", "AdaQP-p"]
 # mode -> (message precision, overlap central aggregation with the exchange)
 QUNAT_PARA_MAP: Dict[str, Tuple[str, bool]] = {"Vanilla": ("full", False), "AdaQP": ("quant", True),
                                                "AdaQP-q": ("quant", False), "AdaQP-p": ("full", True)}
-# 'gat' is an extension beyond the reference's two models
-MODEL_MAP: Dict[str, DistGNNType] = {"gcn": DistGNNType.DistGCN, "sage": DistGNNType.DistSAGE, "gat": DistGNNType.DistGAT}
+# 'gat' and 'appnp' are extensions beyond the reference's two models
+MODEL_MAP: Dict[str, DistGNNType] = {"gcn": DistGNNType.DistGCN, "sage": DistGNNType.DistSAGE, "gat": DistGNNType.DistGAT,
+                                     "appnp": DistGNNType.DistAPPNP}
 GAT_HEADS = 4          # default of the yaml `model: gat_heads`
 
 
@@ -55,6 +57,9 @@ class Trainer(object):
                 self.config["assignment"][k] = args[k]
         model = self.config["model"]
         model["gat_heads"] = int(args["gat_heads"]) if args.get("gat_heads") is not None else int(model.get("gat_heads", GAT_HEADS))
+        # APPNP propagation steps K and teleport probability alpha: run-time value, else the yaml's, else the default
+        for key, default in (("appnp_k", APPNP_K), ("appnp_alpha", APPNP_ALPHA)):
+            model[key] = args[key] if args.get(key) is not None else model.get(key, default)
         if args.get("aggregator_type") is not None:        # extension: run-time override of the yaml's aggregator
             model["aggregator_type"] = args["aggregator_type"]
         rt = self.config["runtime"]
@@ -96,6 +101,11 @@ class Trainer(object):
             if comm.ctx.transport != "p2p":
                 raise NotImplementedError("model 'gat' runs on the p2p transport only; the CPU gloo plumbing mode "
                                           "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports gcn and sage")
+        if self._is_appnp():
+            appnp_params(model["appnp_k"], model["appnp_alpha"])
+            if comm.ctx.transport != "p2p":
+                raise NotImplementedError("model 'appnp' runs on the p2p transport only; the CPU gloo plumbing mode "
+                                          "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports gcn and sage")
         if self._is_pool() and comm.ctx.transport != "p2p":
             raise NotImplementedError("aggregator_type 'pool' runs on the p2p transport only; the CPU gloo plumbing mode "
                                       "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports the mean and gcn aggregators")
@@ -127,6 +137,10 @@ class Trainer(object):
         elif self._is_pool():
             # max-pool exchanges the pooled rows p of every layer (plus backward0 and the arg rows)
             extra["key_dims"] = self._key_dims()
+        elif self._is_appnp():
+            # APPNP exchanges num_classes-wide rows at each of its K steps: one fp32 test{k} buffer per step
+            shape = [data["num_classes"]] * int(model["appnp_k"])
+            extra["key_dims"] = self._key_dims()
         comm.ctx.init_buffer(shape, engine.ctx.send_idx, engine.ctx.recv_idx, engine.ctx.bit_type,
                              total_send_idx=engine.ctx.total_send_idx, num_remote=engine.ctx.num_remove, **extra)
         if self._is_pool():
@@ -144,6 +158,9 @@ class Trainer(object):
     def _is_gat(self) -> bool:
         return MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistGAT
 
+    def _is_appnp(self) -> bool:
+        return MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistAPPNP
+
     def _is_pool(self) -> bool:
         return (MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistSAGE
                 and self.config["model"]["aggregator_type"] == "pool")
@@ -155,6 +172,8 @@ class Trainer(object):
         if self._is_pool():
             data, model = self.config["data"], self.config["model"]
             return sage_pool_key_dims([data["num_feats"]] + [model["hidden_dim"]] * (model["num_layers"] - 1))
+        if self._is_appnp():
+            return appnp_key_dims(self.config["data"]["num_classes"], int(self.config["model"]["appnp_k"]))
         return None
 
     def _gat_shapes(self):
@@ -182,6 +201,8 @@ class Trainer(object):
             self.model = DistGCN(*common).to(comm.ctx.device)
         elif kind == DistGNNType.DistGAT:
             self.model = DistGAT(*common, heads=model["gat_heads"]).to(comm.ctx.device)
+        elif kind == DistGNNType.DistAPPNP:
+            self.model = DistAPPNP(*common, k=model["appnp_k"], alpha=model["appnp_alpha"]).to(comm.ctx.device)
         else:
             self.model = DistSAGE(*common, model["aggregator_type"]).to(comm.ctx.device)
 

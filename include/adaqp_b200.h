@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define ADAQP_ABI_VERSION 5
+#define ADAQP_ABI_VERSION 6
 
 #define ADAQP_EINVAL (-1)   /* bad argument (bits not in {1,2,4,8}, negative size ...) */
 #define ADAQP_EALIGN (-2)   /* pointer alignment requirement violated */
@@ -234,6 +234,23 @@ int adaqp_spmm_csr_seg_f32(const int64_t *indptr, const int64_t *seg_start, cons
                            const float *x1, int64_t ld1, const float *pre, const float *post,
                            int mean, int add_self, int accumulate, int64_t row_begin,
                            int64_t row_end, int32_t F, float *out, int64_t ldo, void *stream);
+
+/* One APPNP personalized-PageRank step (DESIGN §13; host mirror adaqp_b200/appnp.py), with the same sources
+ * (x0 | x1 split at n_split), per-row segments and accumulate mode as adaqp_spmm_csr_seg_f32:
+ *   r[v] = (scale * post[v]) * sum_{u in seg(v)} pre[u] x[u]                v in [row_begin, row_end) <= n_split
+ * forward (tele != NULL):  out[v] = r[v] + alpha * tele[v]            (scale = 1 - alpha, tele = z)
+ * backward (acc_mode != 0, bit 0 set):  a[v] = alpha * x0[v] (+ acc[v] when bit 1 is set);
+ *   without bit 2: out[v] = r[v], acc[v] = a[v];  with bit 2 (fold): out[v] = r[v] + a[v], acc is only read.
+ * tele and acc_mode are exclusive; with neither, out[v] = r[v].  The once-per-row terms (tele, acc) belong
+ * to the call with accumulate == 0: a call with accumulate != 0 (the halo segment of a split row) does
+ * out[v] += r[v] only.  tele / acc / out rows are indexed v - row_begin (pitch ldt / lda / ldo).  fp32, the
+ * __fmaf_rn chain of adaqp_spmm_csr_seg_f32 in CSR order, no float atomics: equal inputs give bitwise equal
+ * outputs.  0 < F <= 1024; rows need only 4-byte alignment (odd F). */
+int adaqp_appnp_prop_f32(const int64_t *indptr, const int64_t *seg_start, const int64_t *seg_end,
+                         const int32_t *indices, const float *x0, int64_t ld0, int64_t n_split, const float *x1,
+                         int64_t ld1, const float *pre, const float *post, float scale, float alpha,
+                         const float *tele, int64_t ldt, float *acc, int64_t lda, int32_t acc_mode, int accumulate,
+                         int64_t row_begin, int64_t row_end, int32_t F, float *out, int64_t ldo, void *stream);
 
 /* --------------------------------------------------------------- dense GEMM
  * C[M, N] = A[M, K] . Bt[N, K]^T (+ bias[N]) in fp32 on the Hopper tensor cores (wgmma) by 3xTF32 error-compensated

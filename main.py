@@ -27,6 +27,10 @@ def parse():
     p.add_argument("--num_epoches", type=int, default=None, help="override the config's epoch count")
     p.add_argument("--aggregator_type", type=str, default=None,
                    help="GraphSAGE aggregator: mean, gcn or pool (default: the config's)")
+    p.add_argument("--appnp_k", type=int, default=None,
+                   help="APPNP propagation steps K (default: the config's `appnp_k`, else 10)")
+    p.add_argument("--appnp_alpha", type=float, default=None,
+                   help="APPNP teleport probability alpha in [0, 1] (default: the config's `appnp_alpha`, else 0.1)")
     p.add_argument("--checkpoint_dir", type=str, default=None,
                    help="directory for epoch checkpoints, `latest` and `best` (the best validation epoch's model)")
     p.add_argument("--checkpoint_every", type=int, default=None, help="write a checkpoint every N epochs (0: off)")
