@@ -96,7 +96,8 @@ def sage_pool_key_dims(widths: Sequence[int]) -> Dict[str, int]:
 def appnp_key_dims(num_classes: int, k: int) -> Dict[str, int]:
     """Exchange keys of APPNP with K propagation steps: step k exchanges h_k on forward{k} (test{k} in evaluation)
     and g_{k+1} on backward{k}; backward0 is needed because the MLP's weight gradients need g_0 at remote
-    destinations.  Every key is num_classes wide."""
+    destinations.  Every key is num_classes wide.  GCNII with L layers uses the same table, hidden_dim wide: layer l
+    exchanges its input on forward{l-1} and its output gradient on backward{l-1}."""
     C = int(num_classes)
     dims = {f"test{i}": C for i in range(k)}
     dims.update({f"forward{i}": C for i in range(k)})

@@ -376,6 +376,104 @@ spmm_csr_sliced_kernel(const int64_t *__restrict__ indptr, const int32_t *__rest
 }
 
 // ---------------------------------------------------------------------------------------
+// Column-sliced propagation step (GCNII's hidden-width rows, DESIGN §14): spmm_csr_sliced_kernel's slice-major
+// schedule and gather with appnp_prop_kernel's epilogue, applied per slice to that slice's columns of tele / acc /
+// x[v] / out.  One destination row per unit (unit = slice * n_rows + row), one float4 of the slice per lane, kUnroll
+// neighbour rows in flight, the weights shuffled after the loads are issued.  The row's own operands are loaded
+// before the gather, and the once-per-row terms belong to the non-accumulating call, as in appnp_prop_kernel.
+// Every output element is the same __fmaf_rn chain in CSR order, followed by the same __fmul_rn(acc, scale * post)
+// and epilogue ops, so the result is bitwise that of appnp_prop_kernel.
+template <int EPI>
+__global__ void __launch_bounds__(kThreads)
+appnp_prop_sliced_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ indices,
+                         const float *__restrict__ x0, int64_t ld0, int64_t n_split,
+                         const float *__restrict__ x1, int64_t ld1,
+                         const float *__restrict__ pre, const float *__restrict__ post, float scale, float alpha,
+                         const float *__restrict__ tele, int64_t ldt, float *__restrict__ accv, int64_t lda, int acc_mode,
+                         int64_t row_begin, int64_t row_end, int F, int slice_cols,
+                         float *__restrict__ out, int64_t ldo, unsigned long long *__restrict__ next_row,
+                         const int64_t *__restrict__ seg_start, const int64_t *__restrict__ seg_end, int accumulate) {
+    const int lane = threadIdx.x & 31;
+    const int64_t n_rows = row_end - row_begin;
+    const int64_t n_units = n_rows * ((F + slice_cols - 1) / slice_cols);
+    const bool once = !accumulate;
+    const bool add_tele = EPI == kEpiTeleport && once && tele != nullptr;
+    const bool acc_on = EPI == kEpiAccum && once && (acc_mode & 1);
+    const bool fold = acc_on && (acc_mode & kAccFold);
+    while (true) {
+        unsigned long long unit = 0;
+        if (lane == 0) unit = atomicAdd(next_row, 1ull);
+        unit = __shfl_sync(ADAQP_FULL_MASK, unit, 0);
+        if ((int64_t)unit >= n_units) break;
+        const int64_t slice = (int64_t)unit / n_rows, o = (int64_t)unit % n_rows;
+        const int col = (int)slice * slice_cols + lane * 4;
+        const bool colok = lane * 4 < slice_cols && col < F;
+        const int64_t row = row_begin + o;
+        float *orow = out + o * ldo + col;
+        float addend[4] = {0.f, 0.f, 0.f, 0.f};
+        if (colok) {
+            if (add_tele) {
+                Vec<4>::load(tele + o * ldt + col, addend);
+            } else if (acc_on) {
+                float own[4];
+                Vec<4>::load(x0 + row * ld0 + col, own);
+                if (acc_mode & kAccRead) Vec<4>::load(accv + o * lda + col, addend);
+#pragma unroll
+                for (int e = 0; e < 4; ++e) addend[e] = __fmaf_rn(alpha, own[e], addend[e]);
+                if (!fold) Vec<4>::store(accv + o * lda + col, addend);
+            } else if (accumulate) {
+                Vec<4>::load(orow, addend);
+            }
+        }
+        const int64_t b = seg_start ? __ldg(seg_start + row) : __ldg(indptr + row);
+        const int64_t e_ = seg_end ? __ldg(seg_end + row) : __ldg(indptr + row + 1);
+        float acc[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int64_t j0 = b; j0 < e_; j0 += 32) {
+            const int n = (e_ - j0) < 32 ? (int)(e_ - j0) : 32;
+            int u = 0;
+            float w = 0.f;
+            if (lane < n) {
+                u = __ldg(indices + j0 + lane);
+                w = pre ? __ldg(pre + u) : 1.f;
+            }
+            for (int k = 0; k < n; k += kUnroll) {
+                float v[kUnroll][4];
+#pragma unroll
+                for (int t = 0; t < kUnroll; ++t) {
+                    const int uu = __shfl_sync(ADAQP_FULL_MASK, u, (k + t) & 31);
+                    const float *rs = (uu < n_split) ? (x0 + (int64_t)uu * ld0) : (x1 + ((int64_t)uu - n_split) * ld1);
+                    if ((k + t) < n && colok) {
+                        Vec<4>::load(rs + col, v[t]);
+                    } else {
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) v[t][e] = 0.f;
+                    }
+                }
+#pragma unroll
+                for (int t = 0; t < kUnroll; ++t) {
+                    float wt = __shfl_sync(ADAQP_FULL_MASK, w, (k + t) & 31);
+                    if ((k + t) >= n) wt = 0.f;
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) acc[e] = __fmaf_rn(wt, v[t][e], acc[e]);
+                }
+            }
+        }
+        if (!colok) continue;
+        const float s = post ? __fmul_rn(scale, __ldg(post + row)) : scale;
+        float r[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            r[e] = __fmul_rn(acc[e], s);
+            if (add_tele) r[e] = __fmaf_rn(alpha, addend[e], r[e]);
+            else if (fold) r[e] = __fadd_rn(r[e], addend[e]);
+            else if (accumulate) r[e] = __fadd_rn(addend[e], r[e]);
+        }
+        Vec<4>::store(orow, r);
+    }
+    frontier_release(next_row);
+}
+
+// ---------------------------------------------------------------------------------------
 // v2: asynchronous row gather through a lane-private shared-memory ring (cp.async / LDGSTS).
 //
 // v1 stages gathered rows in registers: bytes in flight per SM are bounded by the register
@@ -1002,8 +1100,29 @@ int adaqp_appnp_prop_f32(const int64_t *indptr, const int64_t *seg_start, const 
     cudaStream_t s = (cudaStream_t)stream;
     unsigned long long *counter = frontier_counter(dev, s);
     ADAQP_REQUIRE(counter != nullptr, ADAQP_EINVAL, "adaqp_appnp_prop_f32: row counter allocation failed");
-    const int64_t grid = adaqp_frontier_grid(row_end - row_begin, kWarps);
     const bool fwd = tele != nullptr || acc_mode == 0;
+    // column slices of 16-byte rows by the SpMM's rule (auto_slice_cols, or option spmm_slice_cols: >= F = unsliced)
+    int slice = 0;
+    if (vec == 4) {
+        const AdaqpOptions &opt = adaqp_options();
+        slice = opt.spmm_slice_cols > 0 ? opt.spmm_slice_cols : auto_slice_cols(F);
+        if (slice >= F) slice = 0;
+        ADAQP_REQUIRE(slice == 0 || (slice % 4 == 0 && slice <= 128), ADAQP_EINVAL,
+                      "adaqp_appnp_prop_f32: slice width %d is not a multiple of 4 in [4, 128]", slice);
+    }
+    if (slice > 0) {
+        const int64_t units = (row_end - row_begin) * ((F + slice - 1) / slice);
+        const int64_t sgrid = adaqp_frontier_grid(units, kWarps);
+        auto launch_sliced = [&](auto kernel) {
+            kernel<<<(unsigned)sgrid, kThreads, 0, s>>>(indptr, indices, x0, ld0, n_split, x1, ld1, pre, post, scale,
+                                                        alpha, tele, ldt, acc, lda, acc_mode, row_begin, row_end, F,
+                                                        slice, out, ldo, counter, seg_start, seg_end, accumulate);
+        };
+        if (fwd) launch_sliced(appnp_prop_sliced_kernel<kEpiTeleport>);
+        else launch_sliced(appnp_prop_sliced_kernel<kEpiAccum>);
+        return adaqp_check_launch("appnp_prop_sliced_kernel");
+    }
+    const int64_t grid = adaqp_frontier_grid(row_end - row_begin, kWarps);
     auto launch = [&](auto kernel) {
         kernel<<<(unsigned)grid, kThreads, 0, s>>>(indptr, indices, x0, ld0, n_split, x1, ld1, pre, post, scale, alpha,
                                                    tele, ldt, acc, lda, acc_mode, row_begin, row_end, F, out, ldo,

@@ -11,6 +11,7 @@ class DistGNNType(enum.Enum):
     DistSAGE = 1
     DistGAT = 2     # extension beyond the reference
     DistAPPNP = 3   # extension beyond the reference
+    DistGCNII = 4   # extension beyond the reference
 
 
 @enum.unique

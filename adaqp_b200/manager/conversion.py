@@ -39,9 +39,9 @@ def halo_requests(raw: RawPartition, model_type: DistGNNType):
     from_halo = src >= n_in
     h = src[from_halo] - n_in
     v = nnz_dst[from_halo]
-    if model_type is DistGNNType.DistGCN or model_type is DistGNNType.DistAPPNP:
-        # processing.py:90-98: sum_v in_deg[v]^-1/2 * out_deg[h]^-1/2 over halo h -> inner v edges (APPNP weighs
-        # its halo rows by the same norms, scaled by the constant 1 - alpha)
+    if model_type in (DistGNNType.DistGCN, DistGNNType.DistAPPNP, DistGNNType.DistGCNII):
+        # processing.py:90-98: sum_v in_deg[v]^-1/2 * out_deg[h]^-1/2 over halo h -> inner v edges (APPNP and GCNII
+        # weigh their halo rows by the same norms, scaled by the constant 1 - alpha)
         w_f = _clamped_pow(raw.in_degrees[v], -0.5).astype(np.float64)
         fp = np.bincount(h, weights=w_f, minlength=raw.n_halo) * _clamped_pow(raw.out_degrees[n_in:], -0.5)
         w_b = _clamped_pow(raw.out_degrees[v], -0.5).astype(np.float64)

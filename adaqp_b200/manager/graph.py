@@ -100,7 +100,9 @@ def appnp_prop(graph: LocalGraph, x_local: torch.Tensor, x_halo: Optional[torch.
         out[v - row_begin] = scale * post[v] * sum_u pre[u] x[u]  (+ alpha * tele[v - row_begin])
     and, with acc_mode (backward), acc[v - row_begin] = alpha * x[v] (+ acc[..] with ACC_READ), or with ACC_FOLD
     the acc term added to out instead.  `tele`, `acc` and `out` are indexed like out.  part='local' / 'halo' as in
-    spmm(): the halo part accumulates its segment's share into `out` and adds no tele / acc term."""
+    spmm(): the halo part accumulates its segment's share into `out` and adds no tele / acc term.  16-byte rows whose
+    width is a multiple of 128 above 128 run column-sliced (appnp_prop_sliced_kernel, bitwise the same result); option
+    spmm_slice_cols forces a slice width as for spmm()."""
     L = _lib.load()
     row_end = graph.n_inner if row_end is None else int(row_end)
     F = int(x_local.shape[1])

@@ -2,3 +2,4 @@ from .distGCN import DistGCN  # noqa: F401
 from .distSAGE import DistSAGE  # noqa: F401
 from .distGAT import DistGAT  # noqa: F401
 from .distAPPNP import DistAPPNP  # noqa: F401
+from .distGCNII import DistGCNII  # noqa: F401

@@ -440,7 +440,34 @@ class DistAggSAGEPool(Function):
         return dp, None, None, None
 
 
-# ---------------------------------------------------------------- APPNP
+# ---------------------------------------------------------------- APPNP / GCNII propagation steps
+def _teleport_step(name: str, quant: bool, g: LocalGraph, h: Tensor, z: Tensor, alpha: float, is_train: bool) -> Tensor:
+    """out = (1 - alpha) A h + alpha z over the exchange of h on `name` (A with the GCN forward norms): one
+    appnp_prop launch per row range of _gat_propagate's overlap, the teleport term in the kernel's epilogue."""
+    pre, post = g.norm["out_-0.5"], g.norm["in_-0.5"]
+    out = torch.empty_like(z)
+
+    def aggregate(lo, hi, h_halo, _, part=None):
+        appnp_prop(g, h, h_halo, pre, post, 1.0 - alpha, alpha, lo, hi, out[lo:hi], tele=z[lo:hi], part=part)
+
+    _gat_propagate(name, quant, h, None, None, is_train, aggregate, split=True)
+    return out
+
+
+def _accum_step(name: str, quant: bool, g: LocalGraph, grad: Tensor, acc: Tensor, alpha: float, mode: int) -> Tensor:
+    """out = (1 - alpha) A^T grad over the exchange of grad on `name` (the swapped norms), and in the same pass the
+    acc term alpha * grad of each row, stored into / added to `acc` or folded into out per `mode` (ACC_* bits)."""
+    pre, post = g.norm["in_-0.5"], g.norm["out_-0.5"]
+    out = torch.empty_like(grad)
+
+    def aggregate(lo, hi, g_halo, _, part=None):
+        appnp_prop(g, grad, g_halo, pre, post, 1.0 - alpha, alpha, lo, hi, out[lo:hi], acc=acc[lo:hi], acc_mode=mode,
+                   part=part)
+
+    _gat_propagate(name, quant, grad, None, None, True, aggregate, split=True)
+    return out
+
+
 class DistAPPNPProp(Function):
     """K personalized-PageRank steps of APPNP over the halo exchange (an extension beyond the reference):
 
@@ -461,17 +488,10 @@ class DistAPPNPProp(Function):
         eng = engine.ctx
         z = z.contiguous()
         g = graph.full if isinstance(graph, DecompGraph) else graph
-        pre, post = g.norm["out_-0.5"], g.norm["in_-0.5"]
         quant = eng.bit_type == BitType.QUANT and is_train
         h = z
         for step in range(k):
-            out = torch.empty_like(z)
-
-            def aggregate(lo, hi, h_halo, _, part=None, h=h, out=out):
-                appnp_prop(g, h, h_halo, pre, post, 1.0 - alpha, alpha, lo, hi, out[lo:hi], tele=z[lo:hi], part=part)
-
-            _gat_propagate(f"forward{step}", quant, h, None, None, is_train, aggregate, split=True)
-            h = out
+            h = _teleport_step(f"forward{step}", quant, g, h, z, alpha, is_train)
         ctx.graph, ctx.k, ctx.alpha = graph, k, alpha
         return h
 
@@ -480,18 +500,44 @@ class DistAPPNPProp(Function):
         grad = grad_outputs[0].contiguous()
         k, alpha = ctx.k, ctx.alpha
         g = ctx.graph.full if isinstance(ctx.graph, DecompGraph) else ctx.graph
-        pre, post = g.norm["in_-0.5"], g.norm["out_-0.5"]
         quant = engine.ctx.bit_type == BitType.QUANT
         acc = torch.empty_like(grad)             # alpha * sum of the g_{k+1} seen so far
         nxt = grad                               # g_{k+1}
         for step in range(k - 1, -1, -1):
-            out = torch.empty_like(grad)
             mode = ACC_ON | (ACC_READ if step < k - 1 else 0) | (ACC_FOLD if step == 0 else 0)
-
-            def aggregate(lo, hi, g_halo, _, part=None, nxt=nxt, out=out, mode=mode):
-                appnp_prop(g, nxt, g_halo, pre, post, 1.0 - alpha, alpha, lo, hi, out[lo:hi], acc=acc[lo:hi],
-                           acc_mode=mode, part=part)
-
-            _gat_propagate(f"backward{step}", quant, nxt, None, None, True, aggregate, split=True)
-            nxt = out
+            nxt = _accum_step(f"backward{step}", quant, g, nxt, acc, alpha, mode)
         return nxt, None, None, None, None
+
+
+# ---------------------------------------------------------------- GCNII
+class DistGCNIIProp(Function):
+    """The propagation of one GCNII layer over the halo exchange (an extension beyond the reference):
+
+        s = (1 - alpha) A d + alpha h0        A = D^-1/2 A D^-1/2 (the GCN norms)
+
+    with d the layer's (dropped-out) input and h0 the initial representation.  Layer l exchanges d on forward{l}
+    (quantised per mode; test{l} in evaluation) and runs the teleport step, which is the column-sliced
+    appnp_prop_sliced_kernel at hidden widths that are multiples of 128 above 128.  The step is linear in (d, h0), so
+    backward saves nothing: one accumulate step over backward{l} writes dd = (1 - alpha) A^T ds and, in the same
+    pass, dh0 = alpha ds (autograd sums the L layers' dh0).  backward0 is exchanged too: layer 1's gradient flows
+    into h0 and on to the input weights.  Quantisation is the identity in backward (straight-through), as in
+    DistAggConv.  p2p transport only; the layer-0 evaluation cache does not apply (h0 depends on the weights)."""
+
+    @staticmethod
+    def forward(ctx, d: Tensor, h0: Tensor, graph, alpha: float, is_train: bool, layer: int) -> Tensor:
+        if comm.ctx.transport != "p2p":
+            raise NotImplementedError("GCNII runs on the p2p transport only (not the CPU gloo plumbing mode)")
+        g = graph.full if isinstance(graph, DecompGraph) else graph
+        quant = engine.ctx.bit_type == BitType.QUANT and is_train
+        s = _teleport_step(f"forward{layer}", quant, g, d.contiguous(), h0.contiguous(), alpha, is_train)
+        ctx.graph, ctx.alpha, ctx.layer = graph, alpha, layer
+        return s
+
+    @staticmethod
+    def backward(ctx: Any, *grad_outputs: Tuple[Tensor, ...]):
+        ds = grad_outputs[0].contiguous()
+        g = ctx.graph.full if isinstance(ctx.graph, DecompGraph) else ctx.graph
+        quant = engine.ctx.bit_type == BitType.QUANT
+        dh0 = torch.empty_like(ds)
+        dd = _accum_step(f"backward{ctx.layer}", quant, g, ds, dh0, ctx.alpha, ACC_ON)
+        return dd, dh0, None, None, None, None

@@ -32,7 +32,8 @@ RUN_FIELDS = ("dataset", "model_name", "aggregator_type", "gat_heads", "layer_di
               "assign_scheme", "key_dims")
 MODEL_FIELDS = RUN_FIELDS[:5]
 # fields added after format 1 was fixed, compared on resume and on prediction: a manifest written before a field
-# existed reads as null, which is what runs of the models without it record.  `propagation` is APPNP's {k, alpha}.
+# existed reads as null, which is what runs of the models without it record.  `propagation` is APPNP's {k, alpha}
+# and GCNII's {layers, alpha, theta}.
 ADDED_FIELDS = ("propagation",)
 
 
@@ -48,8 +49,17 @@ def run_fields(config: dict, key_dims: Optional[Dict[str, int]]) -> dict:
             "gat_heads": int(model["gat_heads"]), "layer_dims": [int(data["num_feats"])] + [H] * (L - 1) + [int(data["num_classes"])],
             "num_parts": int(rt["num_parts"]), "mode": rt["mode"], "assign_scheme": rt["assign_scheme"],
             "key_dims": {k: int(v) for k, v in key_dims.items()},
-            "propagation": ({"k": int(model["appnp_k"]), "alpha": float(model["appnp_alpha"])}
-                            if rt["model_name"] == "appnp" else None)}
+            "propagation": _propagation(rt["model_name"], model)}
+
+
+def _propagation(model_name: str, model: dict) -> Optional[dict]:
+    """The propagation parameters of the models that have them (None for the others)."""
+    if model_name == "appnp":
+        return {"k": int(model["appnp_k"]), "alpha": float(model["appnp_alpha"])}
+    if model_name == "gcnii":
+        return {"layers": int(model["gcnii_layers"]), "alpha": float(model["gcnii_alpha"]),
+                "theta": float(model["gcnii_theta"])}
+    return None
 
 
 def partition_digest(layout) -> dict:

@@ -22,8 +22,9 @@ from .. import sage_pool
 from ..manager import DecompGraph
 from ..manager import GraphEngine as engine
 from ..communicator.p2p import appnp_key_dims, gat_key_dims, sage_pool_key_dims
-from ..model import DistAPPNP, DistGAT, DistGCN, DistSAGE
+from ..model import DistAPPNP, DistGAT, DistGCN, DistGCNII, DistSAGE
 from ..model.distAPPNP import APPNP_ALPHA, APPNP_K, appnp_params
+from ..model.distGCNII import GCNII_ALPHA, GCNII_LAYERS, GCNII_THETA, gcnii_params
 from ..manager.graphEngine import load_rank_layout
 from ..model.distGAT import gat_layer_shapes
 from . import checkpoint as ckpt
@@ -34,9 +35,9 @@ RUNING_MODE = ["Vanilla", "AdaQP", "AdaQP-q", "AdaQP-p"]
 # mode -> (message precision, overlap central aggregation with the exchange)
 QUNAT_PARA_MAP: Dict[str, Tuple[str, bool]] = {"Vanilla": ("full", False), "AdaQP": ("quant", True),
                                                "AdaQP-q": ("quant", False), "AdaQP-p": ("full", True)}
-# 'gat' and 'appnp' are extensions beyond the reference's two models
+# 'gat', 'appnp' and 'gcnii' are extensions beyond the reference's two models
 MODEL_MAP: Dict[str, DistGNNType] = {"gcn": DistGNNType.DistGCN, "sage": DistGNNType.DistSAGE, "gat": DistGNNType.DistGAT,
-                                     "appnp": DistGNNType.DistAPPNP}
+                                     "appnp": DistGNNType.DistAPPNP, "gcnii": DistGNNType.DistGCNII}
 GAT_HEADS = 4          # default of the yaml `model: gat_heads`
 
 
@@ -59,6 +60,9 @@ class Trainer(object):
         model["gat_heads"] = int(args["gat_heads"]) if args.get("gat_heads") is not None else int(model.get("gat_heads", GAT_HEADS))
         # APPNP propagation steps K and teleport probability alpha: run-time value, else the yaml's, else the default
         for key, default in (("appnp_k", APPNP_K), ("appnp_alpha", APPNP_ALPHA)):
+            model[key] = args[key] if args.get(key) is not None else model.get(key, default)
+        # GCNII layers L, initial-residual weight alpha and identity-mapping strength theta, with the same precedence
+        for key, default in (("gcnii_layers", GCNII_LAYERS), ("gcnii_alpha", GCNII_ALPHA), ("gcnii_theta", GCNII_THETA)):
             model[key] = args[key] if args.get(key) is not None else model.get(key, default)
         if args.get("aggregator_type") is not None:        # extension: run-time override of the yaml's aggregator
             model["aggregator_type"] = args["aggregator_type"]
@@ -106,6 +110,11 @@ class Trainer(object):
             if comm.ctx.transport != "p2p":
                 raise NotImplementedError("model 'appnp' runs on the p2p transport only; the CPU gloo plumbing mode "
                                           "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports gcn and sage")
+        if self._is_gcnii():
+            gcnii_params(model["gcnii_layers"], model["gcnii_alpha"], model["gcnii_theta"])
+            if comm.ctx.transport != "p2p":
+                raise NotImplementedError("model 'gcnii' runs on the p2p transport only; the CPU gloo plumbing mode "
+                                          "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports gcn and sage")
         if self._is_pool() and comm.ctx.transport != "p2p":
             raise NotImplementedError("aggregator_type 'pool' runs on the p2p transport only; the CPU gloo plumbing mode "
                                       "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports the mean and gcn aggregators")
@@ -141,6 +150,10 @@ class Trainer(object):
             # APPNP exchanges num_classes-wide rows at each of its K steps: one fp32 test{k} buffer per step
             shape = [data["num_classes"]] * int(model["appnp_k"])
             extra["key_dims"] = self._key_dims()
+        elif self._is_gcnii():
+            # GCNII exchanges hidden-width rows at each of its L layers: one fp32 test{l} buffer per layer
+            shape = [model["hidden_dim"]] * int(model["gcnii_layers"])
+            extra["key_dims"] = self._key_dims()
         comm.ctx.init_buffer(shape, engine.ctx.send_idx, engine.ctx.recv_idx, engine.ctx.bit_type,
                              total_send_idx=engine.ctx.total_send_idx, num_remote=engine.ctx.num_remove, **extra)
         if self._is_pool():
@@ -161,6 +174,9 @@ class Trainer(object):
     def _is_appnp(self) -> bool:
         return MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistAPPNP
 
+    def _is_gcnii(self) -> bool:
+        return MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistGCNII
+
     def _is_pool(self) -> bool:
         return (MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistSAGE
                 and self.config["model"]["aggregator_type"] == "pool")
@@ -174,6 +190,9 @@ class Trainer(object):
             return sage_pool_key_dims([data["num_feats"]] + [model["hidden_dim"]] * (model["num_layers"] - 1))
         if self._is_appnp():
             return appnp_key_dims(self.config["data"]["num_classes"], int(self.config["model"]["appnp_k"]))
+        if self._is_gcnii():
+            # the same key table as APPNP's: test / forward / backward 0 .. L-1, all hidden_dim wide
+            return appnp_key_dims(self.config["model"]["hidden_dim"], int(self.config["model"]["gcnii_layers"]))
         return None
 
     def _gat_shapes(self):
@@ -203,6 +222,10 @@ class Trainer(object):
             self.model = DistGAT(*common, heads=model["gat_heads"]).to(comm.ctx.device)
         elif kind == DistGNNType.DistAPPNP:
             self.model = DistAPPNP(*common, k=model["appnp_k"], alpha=model["appnp_alpha"]).to(comm.ctx.device)
+        elif kind == DistGNNType.DistGCNII:
+            self.model = DistGCNII(data["num_feats"], model["hidden_dim"], data["num_classes"], model["dropout_rate"],
+                                   layers=model["gcnii_layers"], alpha=model["gcnii_alpha"],
+                                   theta=model["gcnii_theta"]).to(comm.ctx.device)
         else:
             self.model = DistSAGE(*common, model["aggregator_type"]).to(comm.ctx.device)
 

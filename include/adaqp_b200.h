@@ -245,7 +245,9 @@ int adaqp_spmm_csr_seg_f32(const int64_t *indptr, const int64_t *seg_start, cons
  * to the call with accumulate == 0: a call with accumulate != 0 (the halo segment of a split row) does
  * out[v] += r[v] only.  tele / acc / out rows are indexed v - row_begin (pitch ldt / lda / ldo).  fp32, the
  * __fmaf_rn chain of adaqp_spmm_csr_seg_f32 in CSR order, no float atomics: equal inputs give bitwise equal
- * outputs.  0 < F <= 1024; rows need only 4-byte alignment (odd F). */
+ * outputs.  0 < F <= 1024; rows need only 4-byte alignment (odd F).  16-byte rows are aggregated in column slices
+ * by the rule of adaqp_spmm_csr_seg_f32 (128 columns when F is a multiple of 128 above 128; option spmm_slice_cols
+ * forces a width, a multiple of 4 up to 128, >= F = unsliced), with bitwise the same result (DESIGN §14). */
 int adaqp_appnp_prop_f32(const int64_t *indptr, const int64_t *seg_start, const int64_t *seg_end,
                          const int32_t *indices, const float *x0, int64_t ld0, int64_t n_split, const float *x1,
                          int64_t ld1, const float *pre, const float *post, float scale, float alpha,

@@ -31,6 +31,13 @@ def parse():
                    help="APPNP propagation steps K (default: the config's `appnp_k`, else 10)")
     p.add_argument("--appnp_alpha", type=float, default=None,
                    help="APPNP teleport probability alpha in [0, 1] (default: the config's `appnp_alpha`, else 0.1)")
+    p.add_argument("--gcnii_layers", type=int, default=None,
+                   help="GCNII propagation layers L (default: the config's `gcnii_layers`, else 8)")
+    p.add_argument("--gcnii_alpha", type=float, default=None,
+                   help="GCNII initial-residual weight alpha in [0, 1] (default: the config's `gcnii_alpha`, else 0.1)")
+    p.add_argument("--gcnii_theta", type=float, default=None,
+                   help="GCNII identity-mapping strength theta > 0, beta_l = log(theta / l + 1) "
+                        "(default: the config's `gcnii_theta`, else 0.5)")
     p.add_argument("--checkpoint_dir", type=str, default=None,
                    help="directory for epoch checkpoints, `latest` and `best` (the best validation epoch's model)")
     p.add_argument("--checkpoint_every", type=int, default=None, help="write a checkpoint every N epochs (0: off)")

@@ -35,7 +35,8 @@ def run(mode, scheme, bits, seed, args, world):
     t = Trainer(Namespace(dataset=args.dataset, num_parts=world, backend="gloo", init_method="env://",
                           model_name=args.model_name, mode=mode, assign_scheme=scheme, logger_level="WARNING",
                           num_epoches=args.epochs, exp_path="/tmp/adaqp_acc_exp", assign_bits=bits,
-                          aggregator_type=args.aggregator_type, appnp_k=args.appnp_k, appnp_alpha=args.appnp_alpha))
+                          aggregator_type=args.aggregator_type, appnp_k=args.appnp_k, appnp_alpha=args.appnp_alpha,
+                          gcnii_layers=args.gcnii_layers, gcnii_alpha=args.gcnii_alpha, gcnii_theta=args.gcnii_theta))
     if scheme == "adaptive":
         t.assigner.assign_cycle = args.assign_cycle
     t.train()
@@ -80,6 +81,7 @@ def worker(args):
                 delta.setdefault(r["name"], []).append(100 * (r["best_val"] - base[r["seed"]]))
         summary = {"world": world, "epochs": args.epochs, "scale": args.scale, "model": args.model_name,
                    "aggregator_type": args.aggregator_type, "appnp_k": args.appnp_k, "appnp_alpha": args.appnp_alpha,
+                   "gcnii_layers": args.gcnii_layers, "gcnii_alpha": args.gcnii_alpha, "gcnii_theta": args.gcnii_theta,
                    "dataset": args.dataset,
                    "feature_signal": signal, "label_noise": args.label_noise, "calibration": calib, "runs": runs,
                    "vanilla_best_val_mean": float(np.mean(list(base.values()))),
@@ -107,6 +109,9 @@ def main():
     ap.add_argument("--aggregator_type", type=str, default=None, help="GraphSAGE aggregator (default: the config's)")
     ap.add_argument("--appnp_k", type=int, default=None, help="APPNP propagation steps (default: the config's)")
     ap.add_argument("--appnp_alpha", type=float, default=None, help="APPNP teleport probability (default: the config's)")
+    ap.add_argument("--gcnii_layers", type=int, default=None, help="GCNII layers (default: the config's)")
+    ap.add_argument("--gcnii_alpha", type=float, default=None, help="GCNII initial-residual weight (default: the config's)")
+    ap.add_argument("--gcnii_theta", type=float, default=None, help="GCNII identity-mapping strength (default: the config's)")
     ap.add_argument("--assign_cycle", type=int, default=20)
     ap.add_argument("--seeds", type=int, default=3)
     ap.add_argument("--seed0", type=int, default=123)
