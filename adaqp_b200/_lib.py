@@ -115,6 +115,14 @@ SYMBOLS = {
     "adaqp_gat_bwd_f32": (C.c_int, [c_void_p, c_void_p, i64, c_void_p, i64, c_void_p, i64, c_void_p, i64, c_void_p, i64,
                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, i32, i32, i64, i64,
                                     c_void_p, i64, c_void_p, c_void_p, c_void_p]),
+    "adaqp_gatv2_fwd_f32": (C.c_int, [c_void_p, c_void_p, i64, c_void_p, i64, c_void_p, i64, c_void_p, i64, c_void_p,
+                                      i32, i32, i64, i64, c_void_p, i64, c_void_p, c_void_p]),
+    "adaqp_gatv2_bwd_inner_f32": (C.c_int, [c_void_p, c_void_p, i64, c_void_p, i64, c_void_p, i64, c_void_p, i64,
+                                            c_void_p, i64, c_void_p, c_void_p, c_void_p, c_void_p, i64, c_void_p,
+                                            c_void_p, i32, i32, i64, i64, c_void_p, i64, c_void_p, i64, c_void_p, i64,
+                                            c_void_p]),
+    "adaqp_gatv2_bwd_halo_f32": (C.c_int, [c_void_p, c_void_p, c_void_p, i64, c_void_p, i64, c_void_p, i64, c_void_p,
+                                           c_void_p, c_void_p, i32, i32, i64, i64, c_void_p, i64, c_void_p]),
     "adaqp_sage_pool_fwd_f32": (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, i64, c_void_p, i64, c_void_p, i64,
                                           i32, i64, i64, C.c_int, c_void_p, i64, c_void_p, i64, c_void_p]),
     "adaqp_sage_pool_bwd_f32": (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, i64, c_void_p, i64,

@@ -12,7 +12,8 @@ bit assignments) stays on the host process group, as in the reference
 (buffer.py:219-231 all_gather_object).
 
 Layer keys: 'forward{l}', 'backward{l}' (training) and 'test{l}' (evaluation, always fp32,
-buffer.py:32-34 "test" buffers).
+buffer.py:32-34 "test" buffers).  GATv2's 'push{l}' keys run the other way: the holder of a halo row sends it back
+to the row's owner, whose push region has one fp32 row per position of its total_send_idx.
 """
 from __future__ import annotations
 
@@ -105,6 +106,27 @@ def appnp_key_dims(num_classes: int, k: int) -> Dict[str, int]:
     return dims
 
 
+def push_key(layer: int) -> str:
+    """fp32 key of GATv2's pushed halo-row gradients: the holder of a halo row sends the row's source-side gradient
+    back to its owner."""
+    return f"push{layer}"
+
+
+def is_push(key: str) -> bool:
+    return key.startswith("push")
+
+
+def gatv2_key_dims(widths: Sequence[int]) -> Dict[str, int]:
+    """Exchange keys and widths of a GATv2 model whose layer l exchanges rows of zs_l (width widths[l]): test /
+    forward keys of every layer, then the push keys.  zd and the attention logits never leave their rank, so there
+    are no backward keys."""
+    L = len(widths)
+    dims = {f"test{i}": int(widths[i]) for i in range(L)}
+    dims.update({f"forward{i}": int(widths[i]) for i in range(L)})
+    dims.update({push_key(i): int(widths[i]) for i in range(L)})
+    return dims
+
+
 def quantisable(key: str) -> bool:
     """Keys that may travel quantised (training exchanges of layer rows); test, attention and arg keys are fp32."""
     return key.startswith(("forward", "backward"))
@@ -121,8 +143,9 @@ def qsize(n: int, bits: int, F: int) -> int:
 @dataclass
 class SlabLayout:
     """Byte offsets inside one rank's slab.  A pure function of (world size, layer dims,
-    rows received from every peer, num_remote), so every rank can compute every peer's
-    layout from the all-gathered row counts."""
+    rows received from every peer, num_remote, rows sent), so every rank can compute every peer's
+    layout from the all-gathered row counts.  The region of a push key holds `push_rows` rows (the
+    length of total_send_idx), every other key's `num_remote`."""
     world_size: int
     keys: List[str]
     dims: Dict[str, int]
@@ -136,11 +159,12 @@ class SlabLayout:
     work_off: int = 0
     status_off: int = 0
     total: int = 0
+    push_rows: int = 0
 
     @staticmethod
     def build(world_size: int, keys: List[str], dims: Dict[str, int], recv_rows: Dict[int, int],
-              num_remote: int) -> "SlabLayout":
-        L = SlabLayout(world_size, list(keys), dict(dims), dict(recv_rows), int(num_remote))
+              num_remote: int, push_rows: int = 0) -> "SlabLayout":
+        L = SlabLayout(world_size, list(keys), dict(dims), dict(recv_rows), int(num_remote), push_rows=int(push_rows))
         off = 0
         for k in keys:
             L.flag_off[k] = off
@@ -162,7 +186,7 @@ class SlabLayout:
                     L.params_off[(k, p)] = off
                     off += _up(4 * n)
             L.halo_off[k] = off
-            off += _up(4 * F * max(num_remote, 1))
+            off += _up(4 * F * max(push_rows if is_push(k) else num_remote, 1))
         L.total = _up(off, 4096)
         return L
 
@@ -299,6 +323,26 @@ def build_send_items(send_peers: Sequence[int], send_idx: Dict[int, Tuple[int, i
     return out, rel
 
 
+def build_push_items(recv_peers: Sequence[int], recv_idx: Dict[int, np.ndarray],
+                     owner_send_idx: Dict[int, Tuple[int, int]]) -> np.ndarray:
+    """Holder-side work items of a push key (pure host code): for each peer p in recv order, halo row recv_idx[p][j]
+    goes to row lo + j of p's push region, where (lo, hi) = p's send_idx[me], the same rows in the same order as p
+    sent them."""
+    items = np.zeros(int(sum(np.asarray(recv_idx[p]).size for p in recv_peers)), _lib.FP_ITEM_DTYPE)
+    n = 0
+    for ci, p in enumerate(recv_peers):
+        ridx = np.asarray(recv_idx[p], np.int64)
+        lo, hi = owner_send_idx[p]
+        if hi - lo != ridx.size:
+            raise RuntimeError(f"peer {p} sends {hi - lo} rows, {ridx.size} expected")
+        sl = items[n:n + ridx.size]
+        sl["src_row"] = ridx
+        sl["chan"] = ci
+        sl["dst_row"] = lo + np.arange(ridx.size, dtype=np.int64)
+        n += ridx.size
+    return items
+
+
 def build_recv_items(recv_peers: Sequence[int], recv_idx: Dict[int, np.ndarray], bits_from_peer: Dict[int, np.ndarray],
                      F: int) -> Tuple[np.ndarray, Dict[int, Tuple[int, int]]]:
     """Receiver work items (op_util.py:216-235): segment layout as on the sender; row j of a segment
@@ -367,6 +411,7 @@ class PeerExchange:
         self.layouts: Dict[int, SlabLayout] = {}
         self.peer_base: Dict[int, int] = {}
         self.peer_recv_idx: Dict[int, np.ndarray] = {}      # peer -> peer's recv_idx[me]
+        self.peer_send_idx: Dict[int, Tuple[int, int]] = {}  # peer -> peer's send_idx[me]
         self.fp_plans: Dict[str, FpPlan] = {}
         self.quant_plans: Dict[str, QuantPlan] = {}
         self.slab: Optional[Slab] = None
@@ -382,14 +427,18 @@ class PeerExchange:
         return {"rank": self.rank,
                 "recv_rows": {p: int(v.size) for p, v in self.recv_idx.items()},
                 "num_remote": self.num_remote,
-                "recv_idx": self.recv_idx}
+                "recv_idx": self.recv_idx,
+                "send_idx": self.send_idx,
+                "total_send": int(self.total_send_idx.size)}
 
     def allocate(self, metas: List[dict]):
         for m in metas:
             self.layouts[m["rank"]] = SlabLayout.build(self.world_size, self.keys, self.dims,
-                                                       m["recv_rows"], m["num_remote"])
+                                                       m["recv_rows"], m["num_remote"], m["total_send"])
             if m["rank"] != self.rank and self.rank in m["recv_idx"]:
                 self.peer_recv_idx[m["rank"]] = np.asarray(m["recv_idx"][self.rank], np.int64)
+            if m["rank"] != self.rank and self.rank in m["send_idx"]:
+                self.peer_send_idx[m["rank"]] = tuple(int(x) for x in m["send_idx"][self.rank])
         for p, (lo, hi) in self.send_idx.items():
             want = self.layouts[p].recv_rows.get(self.rank, 0)
             if want != hi - lo:
@@ -411,8 +460,11 @@ class PeerExchange:
         return self.slab.ptr + self.layout.work_off + 8 * self.keys.index(key) + 4 * side
 
     def halo(self, key: str) -> torch.Tensor:
+        """The received rows of a key: [num_remote, F], or for a push key the push region [len(total_send_idx), F]
+        (row i holds the gradient pushed for send position i)."""
         F = self.dims[key]
-        return self.slab.view(self.layout.halo_off[key], (self.num_remote, F), torch.float32)
+        rows = self.layout.push_rows if is_push(key) else self.num_remote
+        return self.slab.view(self.layout.halo_off[key], (rows, F), torch.float32)
 
     def recv_region(self, key: str, p: int) -> Tuple[torch.Tensor, torch.Tensor]:
         """(int8[sum q], bf16[2, S]) views of what peer p wrote: the tensors the reference
@@ -432,6 +484,9 @@ class PeerExchange:
     def _build_fp_plans(self):
         me = self.rank
         for key in self.keys:
+            if is_push(key):
+                self._build_push_plan(key)
+                continue
             F = self.dims[key]
             items = np.zeros(int(sum(hi - lo for lo, hi in self.send_idx.values())), _lib.FP_ITEM_DTYPE)
             chans = np.zeros(len(self.send_peers), _lib.SEND_CHAN_DTYPE)
@@ -457,6 +512,26 @@ class PeerExchange:
                 n_items=int(items.size), chans=_to_device_bytes(chans, self.device), n_chans=len(self.send_peers),
                 flags_ptrs=_to_device_bytes(flags, self.device), acks_ptrs=_to_device_bytes(acks, self.device),
                 n_recv=len(self.recv_peers))
+
+    def _build_push_plan(self, key: str):
+        """The roles of _build_fp_plans swapped: I send my halo rows to their owners (my recv peers) and wait on the
+        flags of, and ack, the peers I send to in the forward direction."""
+        me = self.rank
+        items = build_push_items(self.recv_peers, self.recv_idx, self.peer_send_idx)
+        chans = np.zeros(len(self.recv_peers), _lib.SEND_CHAN_DTYPE)
+        for ci, p in enumerate(self.recv_peers):
+            lay_p = self.layouts[p]
+            chans[ci]["fp_rows"] = self.peer_base[p] + lay_p.halo_off[key]
+            chans[ci]["flag"] = self.peer_base[p] + lay_p.flag_off[key] + 4 * me
+            chans[ci]["ack"] = self.slab.ptr + self.layout.ack_off[key] + 4 * p
+            chans[ci]["S"] = self.recv_idx[p].size
+        flags = np.array([self.slab.ptr + self.layout.flag_off[key] + 4 * p for p in self.send_peers], np.uint64)
+        acks = np.array([self.peer_base[p] + self.layouts[p].ack_off[key] + 4 * me for p in self.send_peers], np.uint64)
+        dev_items = _to_device_bytes(items, self.device)
+        self.fp_plans[key] = FpPlan(
+            items=dev_items, items_compat=dev_items, n_items=int(items.size), chans=_to_device_bytes(chans, self.device),
+            n_chans=len(self.recv_peers), flags_ptrs=_to_device_bytes(flags, self.device),
+            acks_ptrs=_to_device_bytes(acks, self.device), n_recv=len(self.send_peers))
 
     # ---- quantised plans ----------------------------------------------------------
     def quant_meta(self, assignment: Dict[str, Dict[int, torch.Tensor]]) -> dict:
@@ -539,6 +614,7 @@ class PeerExchange:
         plan = self.fp_plans[key]
         F = self.dims[key]
         assert x.dtype == torch.float32 and x.shape[1] == F and x.stride(1) == 1
+        assert not (gathered and is_push(key)), "a push key sends the halo rows in place"
         seq = self._next_seq(key)
         items = plan.items_compat if gathered else plan.items
         tok = self._bracket("send", stream)

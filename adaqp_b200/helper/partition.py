@@ -29,7 +29,8 @@ def graph_patition_store(dataset: str, partition_size: int, raw_dir: str = "data
     from adaqp_b200.manager.graphEngine import save_rank_layout
     from adaqp_b200.manager.layout import layouts_from_raw, raw_partitions, save_partition_book
 
-    MODELS = {"gcn": DistGNNType.DistGCN, "sage": DistGNNType.DistSAGE, "gat": DistGNNType.DistGAT}
+    MODELS = {"gcn": DistGNNType.DistGCN, "sage": DistGNNType.DistSAGE, "gat": DistGNNType.DistGAT,
+              "gatv2": DistGNNType.DistGATv2}
     if model_name not in MODELS:
         raise ValueError(f"model_name must be one of {sorted(MODELS)}, got {model_name}")
     if not torch.cuda.is_available():

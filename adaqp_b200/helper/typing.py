@@ -12,6 +12,7 @@ class DistGNNType(enum.Enum):
     DistGAT = 2     # extension beyond the reference
     DistAPPNP = 3   # extension beyond the reference
     DistGCNII = 4   # extension beyond the reference
+    DistGATv2 = 5   # extension beyond the reference
 
 
 @enum.unique

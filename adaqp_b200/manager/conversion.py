@@ -49,7 +49,7 @@ def halo_requests(raw: RawPartition, model_type: DistGNNType):
     elif model_type is DistGNNType.DistSAGE:
         fp = np.bincount(h, weights=_clamped_pow(raw.in_degrees[v], -1).astype(np.float64), minlength=raw.n_halo)
         bp = np.bincount(h, weights=_clamped_pow(raw.out_degrees[v], -1).astype(np.float64), minlength=raw.n_halo)
-    elif model_type is DistGNNType.DistGAT:
+    elif model_type in (DistGNNType.DistGAT, DistGNNType.DistGATv2):
         # static proxy: the attention weights are data-dependent and change every step, so a halo row is scored by
         # the weight it would get under uniform attention, sum_v 1/indeg[v] (the SAGE-mean score); forward rows (z)
         # and backward rows (dL/dout) are both weighed by it

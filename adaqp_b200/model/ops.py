@@ -17,9 +17,9 @@ import torch
 from torch import Tensor
 from torch.autograd import Function
 
-from .. import gat, sage_pool
+from .. import gat, gatv2, sage_pool
 from ..communicator import Communicator as comm
-from ..communicator.p2p import attn_keys, pool_arg_key
+from ..communicator.p2p import attn_keys, pool_arg_key, push_key
 from ..helper import BitType, ProprogationMode
 from ..manager import DecompGraph
 from ..manager import GraphEngine as engine
@@ -386,6 +386,98 @@ class DistAggGAT(Function):
         da_l = (dl.unsqueeze(-1) * zh).sum(0)
         da_r = (dr.unsqueeze(-1) * zh).sum(0)
         return dz, da_l.view_as(a_l), da_r.view_as(a_r), None, None, None, None
+
+
+# ---------------------------------------------------------------- GATv2
+class DistAggGATv2(Function):
+    """GATv2 attention aggregation of local + remote neighbours (an extension beyond the reference).
+
+    forward(zs, zd, attn, graph, layer, is_train, heads) -> out: the exchange moves the source projection zs (key
+    forward{l}, quantised per mode; test{l} in evaluation); zd never leaves its rank.  The received halo zs is copied
+    out of the slab because the backward pass needs it.  The central rows run while the exchange is in flight, the
+    marginal rows in one pass after it lands.  The logit of an edge u -> v needs zs[u] and zd[v] together, so only
+    v's rank can evaluate it: backward computes the source-side gradient of every received halo row
+    (gatv2_bwd_halo), pushes it back to the row's owner in fp32 on push{l} while the central rows run, then runs the
+    marginal rows with the pushed rows folded into dzs.  da is a deterministic torch sum of per-row shares.  The
+    pushed gradient is the straight-through gradient of the (possibly dequantised) halo copy each rank used.  p2p
+    transport only.  The layer-0 evaluation cache never applies: the exchanged rows are zs, not the input
+    features."""
+
+    @staticmethod
+    def forward(ctx, zs: Tensor, zd: Tensor, attn: Tensor, graph, layer: int, is_train: bool, heads: int) -> Tensor:
+        if comm.ctx.transport != "p2p":
+            raise NotImplementedError("GATv2 runs on the p2p transport only (not the CPU gloo plumbing mode)")
+        eng = engine.ctx
+        zs, zd = zs.contiguous(), zd.contiguous()
+        n, F = zs.shape
+        g = graph.full if isinstance(graph, DecompGraph) else graph
+        out = zs.new_empty((n, F))
+        lse = zs.new_empty((n, heads))
+
+        def aggregate(lo, hi, zs_halo, _):
+            if zs_halo is not None and is_train:          # kept for the backward pass; the slab rows are reused
+                zs_halo = zs_halo.clone()
+            gatv2.forward(g, zs, zs_halo, zd, attn, heads, lo, hi, out[lo:hi], lse[lo:hi])
+            return zs_halo
+
+        quant = eng.bit_type == BitType.QUANT and is_train
+        zs_halo = _gat_propagate(f"forward{layer}", quant, zs, None, None, is_train, aggregate)
+        if is_train:
+            if zs_halo is None:
+                zs_halo = zs.new_empty((0, F))
+            ctx.save_for_backward(zs, zs_halo, zd, out, lse, attn)
+            ctx.graph, ctx.layer, ctx.heads = graph, layer, heads
+        return out
+
+    @staticmethod
+    def backward(ctx: Any, *grad_outputs: Tuple[Tensor, ...]):
+        zs, zs_halo, zd, out, lse, attn = ctx.saved_tensors
+        grad = grad_outputs[0].contiguous()
+        heads, layer = ctx.heads, ctx.layer
+        n, F = zs.shape
+        D = F // heads
+        eng, timer, ex = engine.ctx, engine.ctx.timer, comm.ctx.comm_buffer.p2p
+        g = ctx.graph.full if isinstance(ctx.graph, DecompGraph) else ctx.graph
+        S = (grad.view(n, heads, D) * out.view(n, heads, D)).sum(-1).contiguous()
+        halo_indptr, halo_dst = eng.gatv2_halo
+        fold = eng.gatv2_fold
+        key, name = push_key(layer), f"backward{layer}"
+        dzs_halo = gatv2.backward_halo(halo_indptr, halo_dst, zs_halo, zd, grad, lse, S, attn, heads)
+        dzs, dzd, da = (zs.new_empty((n, F)) for _ in range(3))
+
+        def inner(lo, hi, push):
+            gatv2.backward_inner(g, zs, zs_halo, zd, grad, lse, S, attn, heads, push, fold if push is not None else None,
+                                 lo, hi, dzs[lo:hi], dzd[lo:hi], da[lo:hi])
+
+        if not eng.use_parallel:
+            with timer.record_events(f"{name}_communication"):
+                ex.post_send_fp(key, dzs_halo)
+                push = ex.complete_recv_fp(key)
+            with timer.record_events(f"{name}_full_aggregation"):
+                inner(0, n, push)
+            ex.release_fp(key)
+        else:
+            main, side = torch.cuda.current_stream(), eng.marginal_stream
+            ready = torch.cuda.Event()
+            ready.record(main)                   # dzs_halo is produced on the default stream
+            side.wait_event(ready)
+            with timer.record_events(f"{name}_communication", stream=side):
+                ex.post_send_fp(key, dzs_halo, stream=side)
+                push = ex.complete_recv_fp(key, stream=side)
+            landed = torch.cuda.Event(enable_timing=True)
+            landed.record(side)
+            nc = eng.num_central
+            with timer.record_events(f"{name}_central_aggregation"):
+                inner(0, nc, None)               # central rows are sent to no peer, so nothing is pushed to them
+            central_done = torch.cuda.Event(enable_timing=True)
+            central_done.record(main)
+            timer.record_exposed(name, central_done, landed)
+            main.wait_event(landed)
+            with timer.record_events(f"{name}_marginal_aggregation"):
+                inner(nc, n, push)
+            ex.release_fp(key)
+            dzs_halo.record_stream(side)
+        return dzs, dzd, da.sum(0).view_as(attn), None, None, None, None
 
 
 # ---------------------------------------------------------------- SAGE max-pool

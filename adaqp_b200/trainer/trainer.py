@@ -18,11 +18,11 @@ from torch import Tensor
 from ..assigner import Assigner as assigner
 from ..communicator import Communicator as comm
 from ..helper import BitType, DistGNNType
-from .. import sage_pool
+from .. import gatv2, sage_pool
 from ..manager import DecompGraph
 from ..manager import GraphEngine as engine
-from ..communicator.p2p import appnp_key_dims, gat_key_dims, sage_pool_key_dims
-from ..model import DistAPPNP, DistGAT, DistGCN, DistGCNII, DistSAGE
+from ..communicator.p2p import appnp_key_dims, gat_key_dims, gatv2_key_dims, sage_pool_key_dims
+from ..model import DistAPPNP, DistGAT, DistGATv2, DistGCN, DistGCNII, DistSAGE
 from ..model.distAPPNP import APPNP_ALPHA, APPNP_K, appnp_params
 from ..model.distGCNII import GCNII_ALPHA, GCNII_LAYERS, GCNII_THETA, gcnii_params
 from ..manager.graphEngine import load_rank_layout
@@ -35,9 +35,10 @@ RUNING_MODE = ["Vanilla", "AdaQP", "AdaQP-q", "AdaQP-p"]
 # mode -> (message precision, overlap central aggregation with the exchange)
 QUNAT_PARA_MAP: Dict[str, Tuple[str, bool]] = {"Vanilla": ("full", False), "AdaQP": ("quant", True),
                                                "AdaQP-q": ("quant", False), "AdaQP-p": ("full", True)}
-# 'gat', 'appnp' and 'gcnii' are extensions beyond the reference's two models
+# 'gat', 'appnp', 'gcnii' and 'gatv2' are extensions beyond the reference's two models
 MODEL_MAP: Dict[str, DistGNNType] = {"gcn": DistGNNType.DistGCN, "sage": DistGNNType.DistSAGE, "gat": DistGNNType.DistGAT,
-                                     "appnp": DistGNNType.DistAPPNP, "gcnii": DistGNNType.DistGCNII}
+                                     "appnp": DistGNNType.DistAPPNP, "gcnii": DistGNNType.DistGCNII,
+                                     "gatv2": DistGNNType.DistGATv2}
 GAT_HEADS = 4          # default of the yaml `model: gat_heads`
 
 
@@ -100,11 +101,11 @@ class Trainer(object):
             raise ValueError(f"Invalid running mode: {rt['mode']}")
         if rt["model_name"] not in MODEL_MAP:
             raise ValueError(f"Invalid model type: {rt['model_name']}")
-        if MODEL_MAP[rt["model_name"]] == DistGNNType.DistGAT:
+        if MODEL_MAP[rt["model_name"]] in (DistGNNType.DistGAT, DistGNNType.DistGATv2):
             gat_layer_shapes(model["hidden_dim"], data["num_classes"], model["num_layers"], model["gat_heads"])
             if comm.ctx.transport != "p2p":
-                raise NotImplementedError("model 'gat' runs on the p2p transport only; the CPU gloo plumbing mode "
-                                          "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports gcn and sage")
+                raise NotImplementedError(f"model '{rt['model_name']}' runs on the p2p transport only; the CPU gloo "
+                                          "plumbing mode (ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports gcn and sage")
         if self._is_appnp():
             appnp_params(model["appnp_k"], model["appnp_alpha"])
             if comm.ctx.transport != "p2p":
@@ -143,6 +144,10 @@ class Trainer(object):
             # GAT exchanges the projected rows z of every layer (plus backward0 and the attention scalars)
             shape, heads = self._gat_shapes()
             extra["key_dims"] = gat_key_dims(shape, heads)
+        elif self._is_gatv2():
+            # GATv2 exchanges the source projection zs of every layer and pushes its halo gradients back
+            shape, _ = self._gat_shapes()
+            extra["key_dims"] = self._key_dims()
         elif self._is_pool():
             # max-pool exchanges the pooled rows p of every layer (plus backward0 and the arg rows)
             extra["key_dims"] = self._key_dims()
@@ -158,6 +163,8 @@ class Trainer(object):
                              total_send_idx=engine.ctx.total_send_idx, num_remote=engine.ctx.num_remove, **extra)
         if self._is_pool():
             self._set_pool_want()
+        if self._is_gatv2():
+            self._set_gatv2_tables()
 
     def _set_pool_want(self):
         """The backward match table of the max-pool aggregation, aligned with the CSR the kernels read; the peers'
@@ -168,8 +175,21 @@ class Trainer(object):
                                    ex.send_idx, ex.total_send_idx, ex.peer_recv_idx)
         eng.pool_want = torch.from_numpy(want).to(g.device)
 
+    def _set_gatv2_tables(self):
+        """GATv2's backward tables, aligned with the CSR the kernels read: the halo-transposed CSR (the inner
+        destinations of every halo row) and the fold table (the push-region rows of every inner row)."""
+        eng, ex = engine.ctx, comm.ctx.comm_buffer.p2p
+        g = eng.graph.full if isinstance(eng.graph, DecompGraph) else eng.graph
+        hp, hd = gatv2.halo_table(g.indptr.cpu().numpy(), g.indices.cpu().numpy(), g.n_inner, ex.num_remote)
+        fp, fpos = gatv2.fold_table(g.n_inner, ex.send_peers, ex.send_idx, ex.total_send_idx)
+        eng.gatv2_halo = tuple(torch.from_numpy(a).to(g.device) for a in (hp, hd))
+        eng.gatv2_fold = tuple(torch.from_numpy(a).to(g.device) for a in (fp, fpos))
+
     def _is_gat(self) -> bool:
         return MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistGAT
+
+    def _is_gatv2(self) -> bool:
+        return MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistGATv2
 
     def _is_appnp(self) -> bool:
         return MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistAPPNP
@@ -185,6 +205,8 @@ class Trainer(object):
         """Per-key exchange widths of the models with their own exchange protocol (None: the reference's keys)."""
         if self._is_gat():
             return gat_key_dims(*self._gat_shapes())
+        if self._is_gatv2():
+            return gatv2_key_dims(self._gat_shapes()[0])
         if self._is_pool():
             data, model = self.config["data"], self.config["model"]
             return sage_pool_key_dims([data["num_feats"]] + [model["hidden_dim"]] * (model["num_layers"] - 1))
@@ -220,6 +242,8 @@ class Trainer(object):
             self.model = DistGCN(*common).to(comm.ctx.device)
         elif kind == DistGNNType.DistGAT:
             self.model = DistGAT(*common, heads=model["gat_heads"]).to(comm.ctx.device)
+        elif kind == DistGNNType.DistGATv2:
+            self.model = DistGATv2(*common, heads=model["gat_heads"]).to(comm.ctx.device)
         elif kind == DistGNNType.DistAPPNP:
             self.model = DistAPPNP(*common, k=model["appnp_k"], alpha=model["appnp_alpha"]).to(comm.ctx.device)
         elif kind == DistGNNType.DistGCNII:

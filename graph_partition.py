@@ -14,7 +14,7 @@ if __name__ == "__main__":
     parser.add_argument("--raw_dir", type=str, default="data/dataset", help="dir to store raw dataset")
     parser.add_argument("--partition_dir", type=str, default="data/part_data", help="dir to store graph partition")
     parser.add_argument("--partition_size", type=int, default=2, help="graph partition size")
-    parser.add_argument("--model_name", type=str, default="gcn", choices=["gcn", "sage", "gat"],
+    parser.add_argument("--model_name", type=str, default="gcn", choices=["gcn", "sage", "gat", "gatv2"],
                         help="model the files are written for (the adaptive assigner's aggregation scores differ)")
     parser.add_argument("--seed", type=int, default=0, help="partitioner seed")
     args = parser.parse_args()

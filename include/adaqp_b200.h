@@ -318,6 +318,39 @@ int adaqp_gat_bwd_f32(const int64_t *indptr, const int32_t *indices, int64_t n_s
                       const float *a_r, int32_t H, int32_t F, int64_t row_begin, int64_t row_end, float *dz,
                       int64_t lddz, float *del, float *der, void *stream);
 
+/* ------------------------------------------------------------ GATv2 attention
+ * DGL's GATv2Conv aggregation (share_weights=False, negative slope 0.2, no attention dropout) over the halo exchange
+ * (csrc/gatv2.cu, host mirror adaqp_b200/gatv2.py).  Rows, head layouts, per-head scalars and the local / halo
+ * source split are those of the GAT entry points; attn is [H * D].  zd, g, lse and S cover the local rows only.
+ * No float atomics: equal inputs give bitwise equal outputs.
+ *
+ * forward: e[v,u,h] = sum_{c in head h} attn[h,c] LeakyReLU(zs[u,h,c] + zd[v,h,c]) over the CSR row of v,
+ * lse[v,h] = logsumexp_u e[v,u,h], out[v,h,:] = sum_u exp(e[v,u,h] - lse[v,h]) zs[u,h,:]; rows are local. */
+int adaqp_gatv2_fwd_f32(const int64_t *indptr, const int32_t *indices, int64_t n_split, const float *zs0,
+                        int64_t ldzs0, const float *zs1, int64_t ldzs1, const float *zd, int64_t ldzd,
+                        const float *attn, int32_t H, int32_t F, int64_t row_begin, int64_t row_end, float *out,
+                        int64_t ldo, float *lse, void *stream);
+/* backward of the inner rows u (row_end <= n_split) of a symmetric graph, g = dL/dout, S[v,h] = <g[v,h,:],
+ * out[v,h,:]>, t[v,u,h] = alpha[v,u,h] (<g[v,h,:], zs[u,h,:]> - S[v,h]), s = zs[u] + zd[v]:
+ *   dzs[u] = sum_{local v in row u} alpha[v,u] g[v] + t[v,u] attn . LeakyReLU'(s) + pushed rows of u
+ *   dzd[u] = sum_{w in row u} t[u,w] attn . LeakyReLU'(zs[w] + zd[u])
+ *   da[u]  = sum_{w in row u} t[u,w] LeakyReLU(zs[w] + zd[u])       (per-row shares; da is their column sum)
+ * The pushed rows of u are push[fold_pos[k]] for k in [fold_indptr[u], fold_indptr[u+1]), added in that order;
+ * push, fold_indptr and fold_pos are all NULL (no fold) or all given. */
+int adaqp_gatv2_bwd_inner_f32(const int64_t *indptr, const int32_t *indices, int64_t n_split, const float *zs0,
+                              int64_t ldzs0, const float *zs1, int64_t ldzs1, const float *zd, int64_t ldzd,
+                              const float *g, int64_t ldg, const float *lse, const float *S, const float *attn,
+                              const float *push, int64_t ldp, const int64_t *fold_indptr, const int32_t *fold_pos,
+                              int32_t H, int32_t F, int64_t row_begin, int64_t row_end, float *dzs, int64_t lddzs,
+                              float *dzd, int64_t lddzd, float *da, int64_t ldda, void *stream);
+/* backward of the halo rows h in [row_begin, row_end): out[h - row_begin] = sum over the inner destinations v in
+ * halo_dst[halo_indptr[h] .. halo_indptr[h+1]) of alpha[v,h] g[v] + t[v,h] attn . LeakyReLU'(zs1[h] + zd[v]): the
+ * gradient of the received row, which its holder pushes back to the row's owner. */
+int adaqp_gatv2_bwd_halo_f32(const int64_t *halo_indptr, const int32_t *halo_dst, const float *zs1, int64_t ldzs1,
+                             const float *zd, int64_t ldzd, const float *g, int64_t ldg, const float *lse,
+                             const float *S, const float *attn, int32_t H, int32_t F, int64_t row_begin,
+                             int64_t row_end, float *out, int64_t ldo, void *stream);
+
 /* ------------------------------------------------------------ GraphSAGE max-pool aggregation
  * DGL's SAGEConv(aggregator_type='pool') neighbourhood max over the halo exchange (csrc/sage_pool.cu, host mirror
  * adaqp_b200/sage_pool.py); an extension beyond the reference, whose aggregators are mean and gcn.  Rows are
