@@ -61,6 +61,27 @@ template <> struct Vec<1> {
     static __device__ __forceinline__ void store_cs(float *p, const float (&v)[1]) { __stcs(p, v[0]); }
 };
 
+// Row liveness (DESIGN §3, "skipping all-zero source rows"): live[r] = 1 when row r of the local source matrix
+// has an element that compares unequal to 0 (a NaN does), 0 when every element is +0 or -0.  A neighbour u whose
+// row is dead adds __fmaf_rn(w, ±0, acc) == acc to every accumulator as long as w is finite: acc starts at +0 and
+// the chain only produces -0 from a product that underflows to -0, so dropping the term leaves every output
+// element unchanged (at most the sign of a zero result can differ, after such an underflow).
+//
+// compact_live_window: the warp's window of n (<= 32) neighbour ids u and weights w, one per lane, is compacted
+// in place to the neighbours that are kept -- halo sources (u >= n_split, always kept), live local rows, and any
+// neighbour whose weight is not finite (inf * 0 is NaN) -- keeping their CSR order.  Lane i takes the i-th kept
+// neighbour; returns how many were kept.
+__device__ __forceinline__ int compact_live_window(int lane, int n, int64_t n_split, const uint8_t *__restrict__ live,
+                                                   int &u, float &w) {
+    const bool keep = lane < n && ((int64_t)u >= n_split || __ldg(live + u) != 0 || !isfinite(w));
+    const unsigned m = __ballot_sync(ADAQP_FULL_MASK, keep);
+    const int kept = __popc(m);
+    const int src = lane < kept ? (int)__fns(m, 0, lane + 1) : lane;
+    u = __shfl_sync(ADAQP_FULL_MASK, u, src);
+    w = __shfl_sync(ADAQP_FULL_MASK, w, src);
+    return kept;
+}
+
 // One warp's weighted gather over the neighbour segment [b, e_) of a destination row:
 // acc += pre[u] * x[u] in CSR order, one __fmaf_rn per element and neighbour, the row's F floats spread
 // across lanes as VEC-wide vectors (CHUNKS per lane), neighbour ids fetched 32 at a time and broadcast by
@@ -69,15 +90,18 @@ template <> struct Vec<1> {
 // function: expanded in place, spmm_csr_kernel compiles to the same SASS as before appnp_prop_kernel
 // shared it (an inlined function changed its register allocation).  Reads acc, colok, lane, indices,
 // b, e_, x0, ld0, n_split, x1, ld1, pre and hints from the enclosing scope.
-#define ADAQP_GATHER_SEGMENT(UNROLL_) \
+// With SKIP_ (a constant) the 32-id window is first compacted to the neighbours compact_live_window keeps, in CSR
+// order, reading the row-liveness array LIVE_; with SKIP_ false the expansion is the gather without liveness.
+#define ADAQP_GATHER_SEGMENT(UNROLL_, SKIP_, LIVE_) \
         for (int64_t j0 = b; j0 < e_; j0 += 32) {                                                                       \
-            const int n = (e_ - j0) < 32 ? (int)(e_ - j0) : 32;                                                         \
+            int n = (e_ - j0) < 32 ? (int)(e_ - j0) : 32;                                                               \
             int u = 0;                                                                                                  \
             float w = 0.f;                                                                                              \
             if (lane < n) {                                                                                             \
                 u = (hints & kHintIndexStreaming) ? __ldcs(indices + j0 + lane) : __ldg(indices + j0 + lane);           \
                 w = pre ? __ldg(pre + u) : 1.f;                                                                         \
             }                                                                                                           \
+            if constexpr (SKIP_) n = compact_live_window(lane, n, n_split, LIVE_, u, w);                                \
             for (int k = 0; k < n; k += UNROLL_) {                                                                      \
                 float v[UNROLL_][CHUNKS][VEC];                                                                          \
                 float ww[UNROLL_];                                                                                      \
@@ -108,7 +132,9 @@ _Pragma("unroll")                                                               
             }                                                                                                           \
         }
 
-template <int VEC, int CHUNKS>
+// SKIP: the gather leaves out the local source rows that `live` marks all-zero (compact_live_window); the
+// result is the same.  SKIP = false is the kernel without liveness (`live` unused).
+template <int VEC, int CHUNKS, bool SKIP>
 __global__ void __launch_bounds__(kThreads)
 spmm_csr_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ indices,
                 const float *__restrict__ x0, int64_t ld0, int64_t n_split,
@@ -116,7 +142,8 @@ spmm_csr_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ 
                 const float *__restrict__ pre, const float *__restrict__ post,
                 int mean, int add_self, int64_t row_begin, int64_t row_end, int F,
                 float *__restrict__ out, int64_t ldo, unsigned long long *__restrict__ next_row, int rows_per_grab,
-                const int64_t *__restrict__ seg_start, const int64_t *__restrict__ seg_end, int accumulate, int hints) {
+                const int64_t *__restrict__ seg_start, const int64_t *__restrict__ seg_end, int accumulate, int hints,
+                const uint8_t *__restrict__ live) {
     const int lane = threadIdx.x & 31;
     bool colok[CHUNKS];
 #pragma unroll
@@ -145,7 +172,7 @@ spmm_csr_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ 
         const int64_t row_b = __ldg(indptr + row), row_e = __ldg(indptr + row + 1);
         const int64_t b = seg_start ? __ldg(seg_start + row) : row_b;
         const int64_t e_ = seg_end ? __ldg(seg_end + row) : row_e;
-        ADAQP_GATHER_SEGMENT(kUnroll)
+        ADAQP_GATHER_SEGMENT(kUnroll, SKIP, live)
         if (add_self) {
             const float ws = pre ? __ldg(pre + row) : 1.f;
             const float *rp = (row < n_split) ? (x0 + row * ld0) : (x1 + (row - n_split) * ld1);
@@ -257,7 +284,7 @@ appnp_prop_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict_
         const int64_t b = seg_start ? __ldg(seg_start + row) : __ldg(indptr + row);
         const int64_t e_ = seg_end ? __ldg(seg_end + row) : __ldg(indptr + row + 1);
         const int hints = 0;
-        ADAQP_GATHER_SEGMENT(kUnroll)
+        ADAQP_GATHER_SEGMENT(kUnroll, false, nullptr)
         const float s = post ? __fmul_rn(scale, __ldg(post + row)) : scale;
 #pragma unroll
         for (int c = 0; c < CHUNKS; ++c) {
@@ -287,7 +314,8 @@ appnp_prop_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict_
 // flight per lane (the weights are shuffled after the loads are issued: 48 registers, no spills, the
 // same occupancy as spmm_csr_kernel<4, 2>).  Every output element is
 // the same __fmaf_rn chain in CSR order as spmm_csr_kernel's, followed by the same self term, mean,
-// post norm and accumulate, so the results are bitwise those of the unsliced kernel.
+// post norm and accumulate, so the results are bitwise those of the unsliced kernel.  SKIP as in spmm_csr_kernel.
+template <bool SKIP>
 __global__ void __launch_bounds__(kThreads)
 spmm_csr_sliced_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ indices,
                        const float *__restrict__ x0, int64_t ld0, int64_t n_split,
@@ -295,7 +323,8 @@ spmm_csr_sliced_kernel(const int64_t *__restrict__ indptr, const int32_t *__rest
                        const float *__restrict__ pre, const float *__restrict__ post,
                        int mean, int add_self, int64_t row_begin, int64_t row_end, int F, int slice_cols,
                        float *__restrict__ out, int64_t ldo, unsigned long long *__restrict__ next_row, int rows_per_grab,
-                       const int64_t *__restrict__ seg_start, const int64_t *__restrict__ seg_end, int accumulate, int hints) {
+                       const int64_t *__restrict__ seg_start, const int64_t *__restrict__ seg_end, int accumulate, int hints,
+                       const uint8_t *__restrict__ live) {
     const int lane = threadIdx.x & 31;
     const int64_t n_rows = row_end - row_begin;
     const int64_t n_grabs = (n_rows + rows_per_grab - 1) / rows_per_grab;
@@ -316,13 +345,14 @@ spmm_csr_sliced_kernel(const int64_t *__restrict__ indptr, const int32_t *__rest
             const int64_t e_ = seg_end ? __ldg(seg_end + row) : row_e;
             float acc[4] = {0.f, 0.f, 0.f, 0.f};
             for (int64_t j0 = b; j0 < e_; j0 += 32) {
-                const int n = (e_ - j0) < 32 ? (int)(e_ - j0) : 32;
+                int n = (e_ - j0) < 32 ? (int)(e_ - j0) : 32;
                 int u = 0;
                 float w = 0.f;
                 if (lane < n) {
                     u = (hints & kHintIndexStreaming) ? __ldcs(indices + j0 + lane) : __ldg(indices + j0 + lane);
                     w = pre ? __ldg(pre + u) : 1.f;
                 }
+                if constexpr (SKIP) n = compact_live_window(lane, n, n_split, live, u, w);
                 for (int k = 0; k < n; k += kUnroll) {
                     float v[kUnroll][4];
 #pragma unroll
@@ -373,6 +403,28 @@ spmm_csr_sliced_kernel(const int64_t *__restrict__ indptr, const int32_t *__rest
         }
     }
     frontier_release(next_row);
+}
+
+// Row liveness of a [rows, F] fp32 matrix with pitch ld: live[r] = 1 when some x[r, c] != 0 (NaN included), else 0.
+// One warp per row (grid-stride), VEC-wide coalesced loads: one read of the matrix, the answer by warp vote.
+template <int VEC>
+__global__ void __launch_bounds__(kThreads)
+row_live_kernel(const float *__restrict__ x, int64_t ld, int64_t rows, int F, uint8_t *__restrict__ live) {
+    const int lane = threadIdx.x & 31;
+    const int64_t nwarps = (int64_t)gridDim.x * kWarps;
+    for (int64_t r = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); r < rows; r += nwarps) {
+        const float *rp = x + r * ld;
+        bool nz = false;
+#pragma unroll 4
+        for (int c = lane * VEC; c < F; c += 32 * VEC) {
+            float v[VEC];
+            Vec<VEC>::load(rp + c, v);
+#pragma unroll
+            for (int e = 0; e < VEC; ++e) nz |= v[e] != 0.f;
+        }
+        nz = __any_sync(ADAQP_FULL_MASK, nz);
+        if (lane == 0) live[r] = nz ? 1 : 0;
+    }
 }
 
 // ---------------------------------------------------------------------------------------
@@ -928,7 +980,7 @@ int adaqp_spmm_csr_seg_f32(const int64_t *indptr, const int64_t *seg_start, cons
                            const int32_t *indices, const float *x0, int64_t ld0,
                            int64_t n_split, const float *x1, int64_t ld1, const float *pre,
                            const float *post, int mean, int add_self, int accumulate, int64_t row_begin,
-                           int64_t row_end, int32_t F, float *out, int64_t ldo, void *stream) {
+                           int64_t row_end, int32_t F, float *out, int64_t ldo, const uint8_t *live, void *stream) {
     ADAQP_REQUIRE(F > 0 && F <= 1024, ADAQP_ELIMIT, "adaqp_spmm_csr_f32: F=%d outside (0,1024]", F);
     ADAQP_REQUIRE(row_end >= row_begin && row_begin >= 0, ADAQP_EINVAL, "adaqp_spmm_csr_f32: bad row range");
     if (row_end == row_begin) return 0;
@@ -1023,18 +1075,27 @@ int adaqp_spmm_csr_seg_f32(const int64_t *indptr, const int64_t *seg_start, cons
         const int64_t units = ((rows + grab - 1) / grab) * ((F + slice - 1) / slice);
         int64_t grid = (units + kWarps - 1) / kWarps;
         if (grid > cta_cap) grid = cta_cap;
-        spmm_csr_sliced_kernel<<<(unsigned)grid, kThreads, 0, s>>>(indptr, indices, x0, ld0, n_split, x1, ld1, pre, post, mean,
-                                                                   add_self, row_begin, row_end, F, slice, out, ldo, counter, grab,
-                                                                   seg_start, seg_end, accumulate, hints);
+        auto launch_sliced = [&](auto kernel) {
+            kernel<<<(unsigned)grid, kThreads, 0, s>>>(indptr, indices, x0, ld0, n_split, x1, ld1, pre, post, mean, add_self,
+                                                       row_begin, row_end, F, slice, out, ldo, counter, grab, seg_start, seg_end,
+                                                       accumulate, hints, live);
+        };
+        if (live) launch_sliced(spmm_csr_sliced_kernel<true>);
+        else launch_sliced(spmm_csr_sliced_kernel<false>);
         return adaqp_check_launch("spmm_csr_sliced_kernel");
     }
     int64_t grid = (rows + kWarps - 1) / kWarps;
     const int grab_now = grab_rows;
     if (grid > cta_cap) grid = cta_cap;
-#define CALL_SPMM(V, C)                                                                           \
-    spmm_csr_kernel<V, C><<<(unsigned)grid, kThreads, 0, s>>>(indptr, indices, x0, ld0, n_split, x1, \
-                                                             ld1, pre, post, mean, add_self,      \
-                                                             row_begin, row_end, F, out, ldo, counter, grab_now, seg_start, seg_end, accumulate, hints)
+#define CALL_SPMM(V, C)                                                                                                  \
+    do {                                                                                                                 \
+        if (live) spmm_csr_kernel<V, C, true><<<(unsigned)grid, kThreads, 0, s>>>(                                       \
+            indptr, indices, x0, ld0, n_split, x1, ld1, pre, post, mean, add_self, row_begin, row_end, F, out, ldo,      \
+            counter, grab_now, seg_start, seg_end, accumulate, hints, live);                                             \
+        else spmm_csr_kernel<V, C, false><<<(unsigned)grid, kThreads, 0, s>>>(                                           \
+            indptr, indices, x0, ld0, n_split, x1, ld1, pre, post, mean, add_self, row_begin, row_end, F, out, ldo,      \
+            counter, grab_now, seg_start, seg_end, accumulate, hints, nullptr);                                          \
+    } while (0)
     if (vec == 4) {
         if (nchunks <= 1) CALL_SPMM(4, 1);
         else if (nchunks <= 2) CALL_SPMM(4, 2);
@@ -1064,7 +1125,23 @@ int adaqp_spmm_csr_f32(const int64_t *indptr, const int32_t *indices, const floa
                        const float *post, int mean, int add_self, int64_t row_begin,
                        int64_t row_end, int32_t F, float *out, int64_t ldo, void *stream) {
     return adaqp_spmm_csr_seg_f32(indptr, nullptr, nullptr, indices, x0, ld0, n_split, x1, ld1, pre, post, mean,
-                                  add_self, 0, row_begin, row_end, F, out, ldo, stream);
+                                  add_self, 0, row_begin, row_end, F, out, ldo, nullptr, stream);
+}
+
+int adaqp_row_live_f32(const float *x, int64_t ld, int64_t rows, int32_t F, uint8_t *live, void *stream) {
+    ADAQP_REQUIRE(F > 0 && rows >= 0 && ld >= F, ADAQP_EINVAL, "adaqp_row_live_f32: bad shape rows=%lld F=%d ld=%lld",
+                  (long long)rows, F, (long long)ld);
+    if (rows == 0) return 0;
+    ADAQP_REQUIRE(x && live, ADAQP_EINVAL, "adaqp_row_live_f32: null pointer");
+    const int sms = adaqp_sm_count() > 0 ? adaqp_sm_count() : 132;
+    int64_t grid = (rows + kWarps - 1) / kWarps;
+    if (grid > (int64_t)sms * 8) grid = (int64_t)sms * 8;
+    cudaStream_t s = (cudaStream_t)stream;
+    if (F % 4 == 0 && ld % 4 == 0 && aligned(x, 4))
+        row_live_kernel<4><<<(unsigned)grid, kThreads, 0, s>>>(x, ld, rows, F, live);
+    else
+        row_live_kernel<1><<<(unsigned)grid, kThreads, 0, s>>>(x, ld, rows, F, live);
+    return adaqp_check_launch("row_live_kernel");
 }
 
 int adaqp_appnp_prop_f32(const int64_t *indptr, const int64_t *seg_start, const int64_t *seg_end,

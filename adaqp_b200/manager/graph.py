@@ -54,10 +54,13 @@ class LocalGraph(object):
 def spmm(graph: LocalGraph, x_local: torch.Tensor, x_halo: Optional[torch.Tensor],
          pre: Optional[torch.Tensor], post: Optional[torch.Tensor], mean: bool = False,
          add_self: bool = False, row_begin: int = 0, row_end: Optional[int] = None,
-         out: Optional[torch.Tensor] = None, stream=None, part: Optional[str] = None) -> torch.Tensor:
+         out: Optional[torch.Tensor] = None, stream=None, part: Optional[str] = None,
+         live: Optional[torch.Tensor] = None) -> torch.Tensor:
     """out[v - row_begin] = post[v] * sum_u pre[u] x[u]  over the CSR rows [row_begin, row_end).
     part='local': only the local-source neighbours of each row (no halo needed);
-    part='halo' : only the halo-source neighbours, ACCUMULATED into `out`."""
+    part='halo' : only the halo-source neighbours, ACCUMULATED into `out`.
+    live: uint8 per row of x_local from row_live(x_local): the gather skips the all-zero local rows, which add
+    exactly nothing, so the result is the same (None: every source row is read)."""
     L = _lib.load()
     row_end = graph.n_inner if row_end is None else int(row_end)
     F = int(x_local.shape[1])
@@ -76,14 +79,31 @@ def spmm(graph: LocalGraph, x_local: torch.Tensor, x_halo: Optional[torch.Tensor
         accumulate, add_self = 1, False
     elif part is not None:
         raise ValueError(part)
+    if live is not None:
+        assert live.dtype == torch.uint8 and live.is_contiguous() and live.numel() >= graph.n_inner
     rc = L.adaqp_spmm_csr_seg_f32(
         graph.indptr.data_ptr(), seg_start, seg_end, graph.indices.data_ptr(), x_local.data_ptr(),
         x_local.stride(0), graph.n_inner, x_halo.data_ptr() if x_halo is not None else None,
         x_halo.stride(0) if x_halo is not None else 0,
         pre.data_ptr() if pre is not None else None, post.data_ptr() if post is not None else None,
         1 if mean else 0, 1 if add_self else 0, accumulate, int(row_begin), row_end, F, out.data_ptr(),
-        out.stride(0), _lib.stream_ptr(stream))
+        out.stride(0), live.data_ptr() if live is not None else None, _lib.stream_ptr(stream))
     _lib.check(rc, "adaqp_spmm_csr_seg_f32")
+    return out
+
+
+def row_live(x: torch.Tensor, out: Optional[torch.Tensor] = None, stream=None) -> torch.Tensor:
+    """live[r] = any(x[r, :] != 0) as uint8 (a NaN row is live), one read of x on the current (or given) stream:
+    the `live` argument of spmm()."""
+    assert x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1
+    rows, F = int(x.shape[0]), int(x.shape[1])
+    if out is None:
+        out = torch.empty(rows, dtype=torch.uint8, device=x.device)
+    assert out.dtype == torch.uint8 and out.is_contiguous() and out.numel() >= rows
+    if rows == 0:
+        return out
+    rc = _lib.load().adaqp_row_live_f32(x.data_ptr(), x.stride(0), rows, F, out.data_ptr(), _lib.stream_ptr(stream))
+    _lib.check(rc, "adaqp_row_live_f32")
     return out
 
 

@@ -18,7 +18,7 @@ import json
 import os
 from multiprocessing import Event
 from multiprocessing.pool import ThreadPool
-from typing import List, Tuple
+from typing import List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -205,6 +205,9 @@ class GraphEngine(object):
         self.timer = Timer(device=dev)
         self.recorder = Recorder(epoches)
         self._agg_type: str = None
+        # index of the model's output layer (num_layers - 1), set by the Trainer: the backward aggregation of that
+        # layer skips the all-zero gradient rows of the nodes outside the train mask (ops._live_rows); None = off
+        self.top_layer: Optional[int] = None
         GraphEngine.ctx = self
 
     def __repr__(self):

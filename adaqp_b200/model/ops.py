@@ -23,7 +23,7 @@ from ..communicator.p2p import attn_keys, pool_arg_key, push_key
 from ..helper import BitType, ProprogationMode
 from ..manager import DecompGraph
 from ..manager import GraphEngine as engine
-from ..manager.graph import ACC_FOLD, ACC_ON, ACC_READ, LocalGraph, appnp_prop, spmm
+from ..manager.graph import ACC_FOLD, ACC_ON, ACC_READ, LocalGraph, appnp_prop, row_live, spmm
 from ..manager.graphEngine import RowRange
 from .op_util import halo_exchange, msg_all2all_GLOO
 
@@ -35,10 +35,10 @@ def _split(graph, feats: Tensor, x_halo: Tensor = None):
     return g, feats, x_halo
 
 
-def _run(g, x_local, x_halo, pre, post, mean, add_self, lo, hi, out=None, part=None):
+def _run(g, x_local, x_halo, pre, post, mean, add_self, lo, hi, out=None, part=None, live=None):
     if isinstance(g, LocalGraph):
         return spmm(g, x_local, x_halo, pre, post, mean=mean, add_self=add_self, row_begin=lo, row_end=hi, out=out,
-                    part=part)
+                    part=part, live=live)
     from ..manager.graph_cpu import spmm_cpu          # gloo plumbing mode
     res = spmm_cpu(g, x_local, x_halo, pre, post, mean=mean, add_self=add_self, row_begin=lo, row_end=hi)
     if out is not None:
@@ -48,9 +48,10 @@ def _run(g, x_local, x_halo, pre, post, mean, add_self, lo, hi, out=None, part=N
 
 
 def GCN_aggregation(graph, feats: Tensor, mode: ProprogationMode = ProprogationMode.Forward,
-                    x_halo: Tensor = None, out: Tensor = None, part: str = None) -> Tensor:
+                    x_halo: Tensor = None, out: Tensor = None, part: str = None, live: Tensor = None) -> Tensor:
     """out[v] = norm2[v] * sum_{u->v} norm1[u] x[u] with global-degree norms (ops.py:17-32).
-    `feats` may be cat(local, halo) as in the reference, or the local rows with `x_halo`."""
+    `feats` may be cat(local, halo) as in the reference, or the local rows with `x_halo`.  `live`: row liveness
+    of the local rows (graph.row_live), so the gather skips the all-zero ones; the result is the same."""
     g, x_local, x_halo = _split(graph, feats, x_halo)
     lo, hi = (graph.begin, graph.end) if isinstance(graph, RowRange) else (0, g.n_inner)
     if mode == ProprogationMode.Forward:
@@ -59,36 +60,37 @@ def GCN_aggregation(graph, feats: Tensor, mode: ProprogationMode = ProprogationM
         pre, post = g.norm["in_-0.5"], g.norm["out_-0.5"]
     else:
         raise ValueError(f"Invalid mode {mode}")
-    return _run(g, x_local, x_halo, pre, post, False, False, lo, hi, out, part)
+    return _run(g, x_local, x_halo, pre, post, False, False, lo, hi, out, part, live)
 
 
 def SAGE_aggregation(graph, feats: Tensor, mode: ProprogationMode = ProprogationMode.Forward,
-                     aggregator_type="mean", x_halo: Tensor = None, out: Tensor = None, part: str = None) -> Tensor:
+                     aggregator_type="mean", x_halo: Tensor = None, out: Tensor = None, part: str = None,
+                     live: Tensor = None) -> Tensor:
     """ops.py:34-67: 'mean' = mean over in-neighbours (fwd) / sum of x[u]/outdeg[u] (bwd);
     'gcn' = (sum + self) / (indeg + 1) (fwd) / sum + self of x/(outdeg+1) (bwd)."""
     g, x_local, x_halo = _split(graph, feats, x_halo)
     lo, hi = (graph.begin, graph.end) if isinstance(graph, RowRange) else (0, g.n_inner)
     if mode == ProprogationMode.Forward:
         if aggregator_type == "mean":
-            return _run(g, x_local, x_halo, None, None, True, False, lo, hi, out, part)
+            return _run(g, x_local, x_halo, None, None, True, False, lo, hi, out, part, live)
         if aggregator_type == "gcn":
-            return _run(g, x_local, x_halo, None, g.norm["in_+1_-1"], False, True, lo, hi, out, part)
+            return _run(g, x_local, x_halo, None, g.norm["in_+1_-1"], False, True, lo, hi, out, part, live)
     elif mode == ProprogationMode.Backward:
         if aggregator_type == "mean":
-            return _run(g, x_local, x_halo, g.norm["out_-1"], None, False, False, lo, hi, out, part)
+            return _run(g, x_local, x_halo, g.norm["out_-1"], None, False, False, lo, hi, out, part, live)
         if aggregator_type == "gcn":
-            return _run(g, x_local, x_halo, g.norm["out_+1_-1"], None, False, True, lo, hi, out, part)
+            return _run(g, x_local, x_halo, g.norm["out_+1_-1"], None, False, True, lo, hi, out, part, live)
     else:
         raise ValueError(f"Invalid mode {mode}")
     raise ValueError(f"Invalid aggregator_type {aggregator_type}")
 
 
-def _aggregate(class_name: str, graph, x_local, x_halo, mode, out, part=None):
+def _aggregate(class_name: str, graph, x_local, x_halo, mode, out, part=None, live=None):
     if class_name == "DistAggConv":
-        return GCN_aggregation(graph, x_local, mode=mode, x_halo=x_halo, out=out, part=part)
+        return GCN_aggregation(graph, x_local, mode=mode, x_halo=x_halo, out=out, part=part, live=live)
     if class_name == "DistAggSAGE":
         return SAGE_aggregation(graph, x_local, mode=mode, aggregator_type=engine.ctx.agg_type, x_halo=x_halo, out=out,
-                                part=part)
+                                part=part, live=live)
     raise ValueError(f"Invalid class_name {class_name}")
 
 
@@ -164,6 +166,30 @@ def _split_marginal() -> bool:
     return _SPLIT
 
 
+_SKIP = None
+
+
+def _skip_zero_rows() -> bool:
+    """Skip the all-zero gradient rows in the output layer's backward aggregation (default; ADAQP_SKIP_ZERO_ROWS=0
+    reads every row, for A/B runs).  The result is the same either way."""
+    global _SKIP
+    if _SKIP is None:
+        import os
+        _SKIP = os.environ.get("ADAQP_SKIP_ZERO_ROWS", "1") != "0"
+    return _SKIP
+
+
+def _live_rows(local_messages: Tensor, layer: int, mode: ProprogationMode):
+    """Row liveness of the gradient the output layer's backward aggregation reads, or None.  The loss only sees the
+    train rows, so dL/dlogits is exactly zero on every other row, and so is that row of dY W^T, the gradient this
+    aggregation gathers: at ogbn-products' 8 % train share, 92 % of its rows.  Lower layers' gradients pass through
+    LayerNorm and are dense, so they are read as they are."""
+    top = getattr(engine.ctx, "top_layer", None)
+    if mode != ProprogationMode.Backward or layer != top or not local_messages.is_cuda or not _skip_zero_rows():
+        return None
+    return row_live(local_messages)
+
+
 def _finish(ctx, out: Tensor, layer: int, mode: ProprogationMode):
     if mode == ProprogationMode.Forward:
         ctx.saved = layer
@@ -183,7 +209,8 @@ def full_graph_propagation(ctx, local_messages: Tensor, graph, layer: int, is_tr
         with timer.record_events(f"{name}_quantization" if quant else f"{name}_communication"):
             pend = halo_exchange(local_messages, name, is_train)
         with timer.record_events(f"{name}_full_aggregation"):
-            out = _aggregate(class_name, g, local_messages, pend.halo, mode, None)
+            live = _live_rows(local_messages, layer, mode)
+            out = _aggregate(class_name, g, local_messages, pend.halo, mode, None, live=live)
         pend.release()
     else:
         send_messages = local_messages[engine.ctx.total_send_idx]
@@ -225,25 +252,29 @@ def decomposed_graph_propagation(ctx, local_messages: Tensor, graph, layer: int,
     landed.record(side)
     out = local_messages.new_empty((eng.num_inner, local_messages.shape[1]))
     with timer.record_events(f"{name}_central_aggregation"):
-        _aggregate(class_name, graph.central_graph, local_messages, None, mode, out[:eng.num_central])
+        live = _live_rows(local_messages, layer, mode)
+        _aggregate(class_name, graph.central_graph, local_messages, None, mode, out[:eng.num_central], live=live)
     if _split_marginal():
         # the marginal rows' LOCAL-source neighbours do not need the halo either: aggregate them while
         # the exchange is still in flight; only the halo-source segment of each row waits for it
         with timer.record_events(f"{name}_marginal_aggregation_local"):
-            _aggregate(class_name, graph.marginal_graph, local_messages, None, mode, out[eng.num_central:], part="local")
+            _aggregate(class_name, graph.marginal_graph, local_messages, None, mode, out[eng.num_central:],
+                       part="local", live=live)
         overlappable_done = torch.cuda.Event(enable_timing=True)
         overlappable_done.record(main)
         timer.record_exposed(name, overlappable_done, landed)
         main.wait_event(landed)
         with timer.record_events(f"{name}_marginal_aggregation_halo"):
-            _aggregate(class_name, graph.marginal_graph, local_messages, pend.halo, mode, out[eng.num_central:], part="halo")
+            _aggregate(class_name, graph.marginal_graph, local_messages, pend.halo, mode, out[eng.num_central:],
+                       part="halo", live=live)
     else:
         central_done = torch.cuda.Event(enable_timing=True)
         central_done.record(main)
         timer.record_exposed(name, central_done, landed)
         main.wait_event(landed)
         with timer.record_events(f"{name}_marginal_aggregation"):
-            _aggregate(class_name, graph.marginal_graph, local_messages, pend.halo, mode, out[eng.num_central:])
+            _aggregate(class_name, graph.marginal_graph, local_messages, pend.halo, mode, out[eng.num_central:],
+                       live=live)
     pend.release()
     local_messages.record_stream(side)
     return _finish(ctx, out, layer, mode)

@@ -131,6 +131,7 @@ class Trainer(object):
         self.engine = engine(rt["num_epoches"], data["partition_path"], rt["dataset"], precision,
                              MODEL_MAP[rt["model_name"]], use_parallel, layout=layout)
         engine.ctx.agg_type = model["aggregator_type"]
+        engine.ctx.top_layer = model["num_layers"] - 1
         if engine.ctx.use_parallel:
             for g in (engine.ctx.graph, engine.ctx.bwd_graph):
                 g.init_copy_buffers(data["num_feats"], model["hidden_dim"], model["num_layers"], engine.ctx.device)

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define ADAQP_ABI_VERSION 6
+#define ADAQP_ABI_VERSION 7
 
 #define ADAQP_EINVAL (-1)   /* bad argument (bits not in {1,2,4,8}, negative size ...) */
 #define ADAQP_EALIGN (-2)   /* pointer alignment requirement violated */
@@ -228,12 +228,21 @@ int adaqp_spmm_csr_f32(const int64_t *indptr, const int32_t *indices,
  * indptr[v+1]) the halo sources: the local part of the marginal rows can then run while the
  * exchange is still in flight and only the halo part waits for it (a finer overlap than the
  * reference's central / marginal split, ops.py:156-193).  `mean` still divides by the full
- * in-degree indptr[v+1] - indptr[v]; add_self belongs to exactly one of the two calls. */
+ * in-degree indptr[v+1] - indptr[v]; add_self belongs to exactly one of the two calls.
+ * `live` (NULL = every source row is read): uint8 per local source row, 0 where the row of x0 is all
+ * zeros (adaqp_row_live_f32).  The gather then skips the neighbours u < n_split with live[u] == 0 and a
+ * finite pre[u]; they add exactly zero, so the result is the same (DESIGN §3).  Halo sources are always
+ * read.  The opt-in spmm_impl variants 2-4 ignore `live`. */
 int adaqp_spmm_csr_seg_f32(const int64_t *indptr, const int64_t *seg_start, const int64_t *seg_end,
                            const int32_t *indices, const float *x0, int64_t ld0, int64_t n_split,
                            const float *x1, int64_t ld1, const float *pre, const float *post,
                            int mean, int add_self, int accumulate, int64_t row_begin,
-                           int64_t row_end, int32_t F, float *out, int64_t ldo, void *stream);
+                           int64_t row_end, int32_t F, float *out, int64_t ldo, const uint8_t *live,
+                           void *stream);
+
+/* live[r] = 1 if some x[r, c] != 0 (a NaN counts as nonzero), else 0, for r < rows; x is [rows, F] fp32 with
+ * pitch ld.  One coalesced read of x on `stream`. */
+int adaqp_row_live_f32(const float *x, int64_t ld, int64_t rows, int32_t F, uint8_t *live, void *stream);
 
 /* One APPNP personalized-PageRank step (DESIGN §13; host mirror adaqp_b200/appnp.py), with the same sources
  * (x0 | x1 split at n_split), per-row segments and accumulate mode as adaqp_spmm_csr_seg_f32:
