@@ -20,7 +20,7 @@ i32 = C.c_int32
 u64 = C.c_uint64
 u32 = C.c_uint32
 
-ADAQP_ABI_VERSION = 7
+ADAQP_ABI_VERSION = 8
 MAX_PARTS = 64           # ADAQP_MAX_PARTS
 LP_HUB_DEGREE = 256      # ADAQP_LP_HUB_DEGREE
 IPC_HANDLE_BYTES = 64
@@ -84,7 +84,7 @@ SYMBOLS = {
                                      c_void_p, i64, c_void_p]),
     "adaqp_spmm_csr_seg_f32": (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, i64, i64, c_void_p,
                                          i64, c_void_p, c_void_p, C.c_int, C.c_int, C.c_int, i64, i64, i32,
-                                         c_void_p, i64, c_void_p, c_void_p]),
+                                         c_void_p, i64, c_void_p, c_void_p, i64, c_void_p]),
     "adaqp_row_live_f32": (C.c_int, [c_void_p, i64, i64, i32, c_void_p, c_void_p]),
     "adaqp_appnp_prop_f32": (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, i64, i64, c_void_p, i64,
                                        c_void_p, c_void_p, C.c_float, C.c_float, c_void_p, i64, c_void_p, i64, i32,

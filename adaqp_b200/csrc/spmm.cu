@@ -134,7 +134,10 @@ _Pragma("unroll")                                                               
 
 // SKIP: the gather leaves out the local source rows that `live` marks all-zero (compact_live_window); the
 // result is the same.  SKIP = false is the kernel without liveness (`live` unused).
-template <int VEC, int CHUNKS, bool SKIP>
+// LIST: only the destination rows rows[0 .. n_list) are computed (absolute CSR row ids in [row_begin, row_end),
+// ascending): the frontier numbers positions in the list instead of rows, and each listed row is computed and
+// stored exactly as without the list; the other output rows are not touched.  LIST = false: `rows` unused.
+template <int VEC, int CHUNKS, bool SKIP, bool LIST>
 __global__ void __launch_bounds__(kThreads)
 spmm_csr_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ indices,
                 const float *__restrict__ x0, int64_t ld0, int64_t n_split,
@@ -143,7 +146,7 @@ spmm_csr_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ 
                 int mean, int add_self, int64_t row_begin, int64_t row_end, int F,
                 float *__restrict__ out, int64_t ldo, unsigned long long *__restrict__ next_row, int rows_per_grab,
                 const int64_t *__restrict__ seg_start, const int64_t *__restrict__ seg_end, int accumulate, int hints,
-                const uint8_t *__restrict__ live) {
+                const uint8_t *__restrict__ live, const int32_t *__restrict__ rows, int64_t n_list) {
     const int lane = threadIdx.x & 31;
     bool colok[CHUNKS];
 #pragma unroll
@@ -154,14 +157,17 @@ spmm_csr_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ 
     // rows) however uneven the degrees are.  With a static row -> warp map the warps drift
     // apart (power-law degrees) and the set of source rows being reused grows far beyond
     // L2, even on graphs where most edges stay inside small communities.
-    const int64_t n_rows = row_end - row_begin;
+    // With LIST the counter walks list positions: position i is row rows[i].
+    const int64_t n_rows = LIST ? n_list : row_end - row_begin;
+    const int64_t pos_base = LIST ? 0 : row_begin;
     while (true) {
         unsigned long long grab = 0;
         if (lane == 0) grab = atomicAdd(next_row, (unsigned long long)rows_per_grab);
         grab = __shfl_sync(ADAQP_FULL_MASK, grab, 0);
         if ((int64_t)grab >= n_rows) break;
         const int64_t r_hi = ((int64_t)grab + rows_per_grab < n_rows) ? (int64_t)grab + rows_per_grab : n_rows;
-    for (int64_t row = row_begin + (int64_t)grab; row < row_begin + r_hi; ++row) {
+    for (int64_t pos = pos_base + (int64_t)grab; pos < pos_base + r_hi; ++pos) {
+        const int64_t row = LIST ? (int64_t)__ldg(rows + pos) : pos;
         float acc[CHUNKS][VEC];
 #pragma unroll
         for (int c = 0; c < CHUNKS; ++c)
@@ -314,8 +320,9 @@ appnp_prop_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict_
 // flight per lane (the weights are shuffled after the loads are issued: 48 registers, no spills, the
 // same occupancy as spmm_csr_kernel<4, 2>).  Every output element is
 // the same __fmaf_rn chain in CSR order as spmm_csr_kernel's, followed by the same self term, mean,
-// post norm and accumulate, so the results are bitwise those of the unsliced kernel.  SKIP as in spmm_csr_kernel.
-template <bool SKIP>
+// post norm and accumulate, so the results are bitwise those of the unsliced kernel.  SKIP and LIST as in
+// spmm_csr_kernel; with LIST the units are (slice, list grab), slice-major.
+template <bool SKIP, bool LIST>
 __global__ void __launch_bounds__(kThreads)
 spmm_csr_sliced_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ indices,
                        const float *__restrict__ x0, int64_t ld0, int64_t n_split,
@@ -324,9 +331,10 @@ spmm_csr_sliced_kernel(const int64_t *__restrict__ indptr, const int32_t *__rest
                        int mean, int add_self, int64_t row_begin, int64_t row_end, int F, int slice_cols,
                        float *__restrict__ out, int64_t ldo, unsigned long long *__restrict__ next_row, int rows_per_grab,
                        const int64_t *__restrict__ seg_start, const int64_t *__restrict__ seg_end, int accumulate, int hints,
-                       const uint8_t *__restrict__ live) {
+                       const uint8_t *__restrict__ live, const int32_t *__restrict__ rows, int64_t n_list) {
     const int lane = threadIdx.x & 31;
-    const int64_t n_rows = row_end - row_begin;
+    const int64_t n_rows = LIST ? n_list : row_end - row_begin;
+    const int64_t pos_begin = LIST ? 0 : row_begin, pos_end = LIST ? n_list : row_end;
     const int64_t n_grabs = (n_rows + rows_per_grab - 1) / rows_per_grab;
     const int64_t n_units = n_grabs * ((F + slice_cols - 1) / slice_cols);
     while (true) {
@@ -337,9 +345,10 @@ spmm_csr_sliced_kernel(const int64_t *__restrict__ indptr, const int32_t *__rest
         const int64_t slice = (int64_t)unit / n_grabs, grab = (int64_t)unit % n_grabs;
         const int col = (int)slice * slice_cols + lane * 4;
         const bool colok = lane * 4 < slice_cols && col < F;
-        const int64_t r_lo = row_begin + grab * rows_per_grab;
-        const int64_t r_hi = (r_lo + rows_per_grab < row_end) ? r_lo + rows_per_grab : row_end;
-        for (int64_t row = r_lo; row < r_hi; ++row) {
+        const int64_t r_lo = pos_begin + grab * rows_per_grab;
+        const int64_t r_hi = (r_lo + rows_per_grab < pos_end) ? r_lo + rows_per_grab : pos_end;
+        for (int64_t pos = r_lo; pos < r_hi; ++pos) {
+            const int64_t row = LIST ? (int64_t)__ldg(rows + pos) : pos;
             const int64_t row_b = __ldg(indptr + row), row_e = __ldg(indptr + row + 1);
             const int64_t b = seg_start ? __ldg(seg_start + row) : row_b;
             const int64_t e_ = seg_end ? __ldg(seg_end + row) : row_e;
@@ -980,10 +989,16 @@ int adaqp_spmm_csr_seg_f32(const int64_t *indptr, const int64_t *seg_start, cons
                            const int32_t *indices, const float *x0, int64_t ld0,
                            int64_t n_split, const float *x1, int64_t ld1, const float *pre,
                            const float *post, int mean, int add_self, int accumulate, int64_t row_begin,
-                           int64_t row_end, int32_t F, float *out, int64_t ldo, const uint8_t *live, void *stream) {
+                           int64_t row_end, int32_t F, float *out, int64_t ldo, const uint8_t *live,
+                           const int32_t *rows, int64_t n_list, void *stream) {
     ADAQP_REQUIRE(F > 0 && F <= 1024, ADAQP_ELIMIT, "adaqp_spmm_csr_f32: F=%d outside (0,1024]", F);
     ADAQP_REQUIRE(row_end >= row_begin && row_begin >= 0, ADAQP_EINVAL, "adaqp_spmm_csr_f32: bad row range");
+    ADAQP_REQUIRE(!rows || (n_list >= 0 && n_list <= row_end - row_begin), ADAQP_EINVAL,
+                  "adaqp_spmm_csr_seg_f32: row list of %lld ids for a range of %lld rows", (long long)n_list,
+                  (long long)(row_end - row_begin));
+    ADAQP_REQUIRE(!(rows && live), ADAQP_EINVAL, "adaqp_spmm_csr_seg_f32: a row list and row liveness together");
     if (row_end == row_begin) return 0;
+    if (rows && n_list == 0) return 0;      // nothing listed: no launch (a grid of 0 is an error), counter untouched
     ADAQP_REQUIRE(indptr && indices && x0 && out, ADAQP_EINVAL, "adaqp_spmm_csr_f32: null pointer");
     int vec = 4;
     auto fits = [&](int v) {
@@ -994,20 +1009,20 @@ int adaqp_spmm_csr_seg_f32(const int64_t *indptr, const int64_t *seg_start, cons
     };
     while (vec > 1 && !fits(vec)) vec >>= 1;
     const int nchunks = (F + 32 * vec - 1) / (32 * vec);
-    const int64_t rows = row_end - row_begin;
+    const int64_t n_rows = row_end - row_begin;
     const int sms = adaqp_sm_count() > 0 ? adaqp_sm_count() : 132;
     const AdaqpOptions &opt = adaqp_options();
     cudaStream_t s = (cudaStream_t)stream;
     const int impl = opt.spmm_impl;
     // v2 (cp.async ring) needs 16-byte rows: F % 4 == 0, strides % 4 == 0, 16-byte aligned bases
-    if (impl == 2 && vec == 4 && nchunks <= 8 && !seg_start && !seg_end && !accumulate) {
+    if (impl == 2 && !rows && vec == 4 && nchunks <= 8 && !seg_start && !seg_end && !accumulate) {
         auto launch = [&](auto kernel, int C) {
             const size_t smem = (size_t)kWarps * kStages * C * 512;
             int ctas_per_sm = (int)((200 * 1024) / (smem + 1024));
             if (ctas_per_sm > 4) ctas_per_sm = 4;
             if (ctas_per_sm < 1) ctas_per_sm = 1;
             int64_t g2 = (int64_t)sms * ctas_per_sm;
-            const int64_t max_ctas = (rows + kWarps - 1) / kWarps;
+            const int64_t max_ctas = (n_rows + kWarps - 1) / kWarps;
             if (g2 > max_ctas) g2 = max_ctas;
             const int64_t chunk_nnz = 2048;   // nnz-balanced work units, many per warp
             cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
@@ -1027,7 +1042,7 @@ int adaqp_spmm_csr_seg_f32(const int64_t *indptr, const int64_t *seg_start, cons
     unsigned long long *counter = frontier_counter(dev, s);
     ADAQP_REQUIRE(counter != nullptr, ADAQP_EINVAL, "adaqp_spmm_csr_seg_f32: row counter allocation failed");
     // v3 / v4 (TMA ring): one TMA box per row -> F <= 256, 16-byte rows
-    if ((impl == 3 || impl == 4) && vec == 4 && F <= 256 && nchunks <= 2) {
+    if ((impl == 3 || impl == 4) && !rows && vec == 4 && F <= 256 && nchunks <= 2) {
         CUtensorMap map0, map1;
         memset(&map0, 0, sizeof(map0));
         memset(&map1, 0, sizeof(map1));
@@ -1044,7 +1059,7 @@ int adaqp_spmm_csr_seg_f32(const int64_t *indptr, const int64_t *seg_start, cons
         if (stages > 8) stages = 8;
         ADAQP_REQUIRE(stages >= 2, ADAQP_ELIMIT, "adaqp_spmm_csr_seg_f32: ring does not fit shared memory");
         const size_t smem = (size_t)kRingWarps * stages * (slot_bytes + sizeof(RingMeta) + 8);
-        int64_t grid = (rows + kRingWarps - 1) / kRingWarps;
+        int64_t grid = (n_rows + kRingWarps - 1) / kRingWarps;
         if (grid > sms) grid = sms;
         const int grab = opt.spmm_rows_per_grab > 0 ? opt.spmm_rows_per_grab : 4;
         auto launch = [&](auto kernel) {
@@ -1070,31 +1085,37 @@ int adaqp_spmm_csr_seg_f32(const int64_t *indptr, const int64_t *seg_start, cons
     // one row per grab (option spmm_rows_per_grab overrides): the narrowest window of rows in flight, so most
     // of the reused source rows stay in L2 (DESIGN §3: 1 row beat 2 by 4 % at F = 256 sliced, 3 % at F = 100)
     const int grab_rows = opt.spmm_rows_per_grab > 0 ? opt.spmm_rows_per_grab : 1;
+    // the rows the launch computes: the list, or the whole range; the grid comes from them
+    const int64_t work_rows = rows ? n_list : n_rows;
     if (slice > 0) {
         const int grab = grab_rows;
-        const int64_t units = ((rows + grab - 1) / grab) * ((F + slice - 1) / slice);
+        const int64_t units = ((work_rows + grab - 1) / grab) * ((F + slice - 1) / slice);
         int64_t grid = (units + kWarps - 1) / kWarps;
         if (grid > cta_cap) grid = cta_cap;
         auto launch_sliced = [&](auto kernel) {
             kernel<<<(unsigned)grid, kThreads, 0, s>>>(indptr, indices, x0, ld0, n_split, x1, ld1, pre, post, mean, add_self,
                                                        row_begin, row_end, F, slice, out, ldo, counter, grab, seg_start, seg_end,
-                                                       accumulate, hints, live);
+                                                       accumulate, hints, live, rows, n_list);
         };
-        if (live) launch_sliced(spmm_csr_sliced_kernel<true>);
-        else launch_sliced(spmm_csr_sliced_kernel<false>);
+        if (rows) launch_sliced(spmm_csr_sliced_kernel<false, true>);
+        else if (live) launch_sliced(spmm_csr_sliced_kernel<true, false>);
+        else launch_sliced(spmm_csr_sliced_kernel<false, false>);
         return adaqp_check_launch("spmm_csr_sliced_kernel");
     }
-    int64_t grid = (rows + kWarps - 1) / kWarps;
+    int64_t grid = (work_rows + kWarps - 1) / kWarps;
     const int grab_now = grab_rows;
     if (grid > cta_cap) grid = cta_cap;
 #define CALL_SPMM(V, C)                                                                                                  \
     do {                                                                                                                 \
-        if (live) spmm_csr_kernel<V, C, true><<<(unsigned)grid, kThreads, 0, s>>>(                                       \
+        if (rows) spmm_csr_kernel<V, C, false, true><<<(unsigned)grid, kThreads, 0, s>>>(                                \
             indptr, indices, x0, ld0, n_split, x1, ld1, pre, post, mean, add_self, row_begin, row_end, F, out, ldo,      \
-            counter, grab_now, seg_start, seg_end, accumulate, hints, live);                                             \
-        else spmm_csr_kernel<V, C, false><<<(unsigned)grid, kThreads, 0, s>>>(                                           \
+            counter, grab_now, seg_start, seg_end, accumulate, hints, nullptr, rows, n_list);                            \
+        else if (live) spmm_csr_kernel<V, C, true, false><<<(unsigned)grid, kThreads, 0, s>>>(                           \
             indptr, indices, x0, ld0, n_split, x1, ld1, pre, post, mean, add_self, row_begin, row_end, F, out, ldo,      \
-            counter, grab_now, seg_start, seg_end, accumulate, hints, nullptr);                                          \
+            counter, grab_now, seg_start, seg_end, accumulate, hints, live, nullptr, 0);                                 \
+        else spmm_csr_kernel<V, C, false, false><<<(unsigned)grid, kThreads, 0, s>>>(                                    \
+            indptr, indices, x0, ld0, n_split, x1, ld1, pre, post, mean, add_self, row_begin, row_end, F, out, ldo,      \
+            counter, grab_now, seg_start, seg_end, accumulate, hints, nullptr, nullptr, 0);                              \
     } while (0)
     if (vec == 4) {
         if (nchunks <= 1) CALL_SPMM(4, 1);
@@ -1125,7 +1146,7 @@ int adaqp_spmm_csr_f32(const int64_t *indptr, const int32_t *indices, const floa
                        const float *post, int mean, int add_self, int64_t row_begin,
                        int64_t row_end, int32_t F, float *out, int64_t ldo, void *stream) {
     return adaqp_spmm_csr_seg_f32(indptr, nullptr, nullptr, indices, x0, ld0, n_split, x1, ld1, pre, post, mean,
-                                  add_self, 0, row_begin, row_end, F, out, ldo, nullptr, stream);
+                                  add_self, 0, row_begin, row_end, F, out, ldo, nullptr, nullptr, 0, stream);
 }
 
 int adaqp_row_live_f32(const float *x, int64_t ld, int64_t rows, int32_t F, uint8_t *live, void *stream) {

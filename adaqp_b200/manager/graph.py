@@ -51,22 +51,78 @@ class LocalGraph(object):
         return self if torch.device(device) == self.device else NotImplemented
 
 
+class RowList(object):
+    """A device list of destination rows for spmm(..., rows=): int32 CSR row ids, ascending and unique, with their
+    bounds kept on the host (`first`, `last`; None when empty), so a launch can check its range without reading
+    the device.  Built by row_list(); `below(n)` / `from_(n)` are the views of the ids < n and >= n."""
+
+    def __init__(self, ids: torch.Tensor, host: np.ndarray):
+        assert ids.dtype == torch.int32 and ids.dim() == 1 and ids.is_contiguous() and ids.numel() == host.size
+        self.ids, self._host = ids, host
+        self.n = int(host.size)
+        self.first = int(host[0]) if self.n else None
+        self.last = int(host[-1]) if self.n else None
+
+    def _cut(self, k: int) -> int:
+        return int(np.searchsorted(self._host, k, side="left"))
+
+    def below(self, n: int) -> "RowList":
+        k = self._cut(n)
+        return RowList(self.ids[:k], self._host[:k])
+
+    def from_(self, n: int) -> "RowList":
+        k = self._cut(n)
+        return RowList(self.ids[k:], self._host[k:])
+
+    def __len__(self) -> int:
+        return self.n
+
+
+def row_list(mask: torch.Tensor, n_rows: int, device) -> RowList:
+    """The rows a mask selects among [0, n_rows) as a RowList on `device`: a bool mask of n_rows entries, or an
+    index tensor (any integer type, duplicates and order allowed).  Built on the host once; ids outside
+    [0, n_rows) are refused."""
+    m = mask.detach().cpu()
+    if m.dtype == torch.bool:
+        if m.dim() != 1 or m.numel() != n_rows:
+            raise ValueError(f"bool row mask of shape {tuple(m.shape)} for {n_rows} rows")
+        host = torch.nonzero(m).flatten().numpy().astype(np.int64)
+    else:
+        if m.is_floating_point() or m.is_complex():
+            raise ValueError(f"row mask of dtype {m.dtype}: a bool mask or integer row ids")
+        host = np.unique(m.flatten().to(torch.int64).numpy())
+    if host.size and (host[0] < 0 or host[-1] >= n_rows):
+        raise ValueError(f"row ids [{int(host[0])}, {int(host[-1])}] outside [0, {n_rows})")
+    host = host.astype(np.int32)
+    return RowList(torch.from_numpy(host).to(device), host)
+
+
 def spmm(graph: LocalGraph, x_local: torch.Tensor, x_halo: Optional[torch.Tensor],
          pre: Optional[torch.Tensor], post: Optional[torch.Tensor], mean: bool = False,
          add_self: bool = False, row_begin: int = 0, row_end: Optional[int] = None,
          out: Optional[torch.Tensor] = None, stream=None, part: Optional[str] = None,
-         live: Optional[torch.Tensor] = None) -> torch.Tensor:
+         live: Optional[torch.Tensor] = None, rows: Optional[RowList] = None) -> torch.Tensor:
     """out[v - row_begin] = post[v] * sum_u pre[u] x[u]  over the CSR rows [row_begin, row_end).
     part='local': only the local-source neighbours of each row (no halo needed);
     part='halo' : only the halo-source neighbours, ACCUMULATED into `out`.
     live: uint8 per row of x_local from row_live(x_local): the gather skips the all-zero local rows, which add
-    exactly nothing, so the result is the same (None: every source row is read)."""
+    exactly nothing, so the result is the same (None: every source row is read).
+    rows: a RowList inside [row_begin, row_end): only those rows of `out` are computed (each exactly as without
+    the list), the others are left as they are; an empty list launches nothing."""
     L = _lib.load()
     row_end = graph.n_inner if row_end is None else int(row_end)
     F = int(x_local.shape[1])
     assert x_local.dtype == torch.float32 and x_local.stride(1) == 1
     if out is None:
         out = torch.empty((row_end - row_begin, F), dtype=torch.float32, device=x_local.device)
+    n_list = 0
+    if rows is not None:
+        assert live is None, "a row list and row liveness are not combined"
+        assert rows.ids.dtype == torch.int32 and rows.ids.is_contiguous() and rows.ids.device == x_local.device
+        if rows.n == 0:
+            return out
+        assert row_begin <= rows.first and rows.last < row_end, (rows.first, rows.last, row_begin, row_end)
+        n_list = rows.n
     if x_halo is not None and x_halo.shape[0] == 0:
         x_halo = None
     seg_start = seg_end = None
@@ -87,7 +143,8 @@ def spmm(graph: LocalGraph, x_local: torch.Tensor, x_halo: Optional[torch.Tensor
         x_halo.stride(0) if x_halo is not None else 0,
         pre.data_ptr() if pre is not None else None, post.data_ptr() if post is not None else None,
         1 if mean else 0, 1 if add_self else 0, accumulate, int(row_begin), row_end, F, out.data_ptr(),
-        out.stride(0), live.data_ptr() if live is not None else None, _lib.stream_ptr(stream))
+        out.stride(0), live.data_ptr() if live is not None else None,
+        rows.ids.data_ptr() if rows is not None else None, n_list, _lib.stream_ptr(stream))
     _lib.check(rc, "adaqp_spmm_csr_seg_f32")
     return out
 

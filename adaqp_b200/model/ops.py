@@ -11,7 +11,8 @@ aggregate on the default stream; ordering is by CUDA events only.
 """
 from __future__ import annotations
 
-from typing import Any, Tuple
+import contextlib
+from typing import Any, Optional, Tuple
 
 import torch
 from torch import Tensor
@@ -23,7 +24,7 @@ from ..communicator.p2p import attn_keys, pool_arg_key, push_key
 from ..helper import BitType, ProprogationMode
 from ..manager import DecompGraph
 from ..manager import GraphEngine as engine
-from ..manager.graph import ACC_FOLD, ACC_ON, ACC_READ, LocalGraph, appnp_prop, row_live, spmm
+from ..manager.graph import ACC_FOLD, ACC_ON, ACC_READ, LocalGraph, RowList, appnp_prop, row_list, row_live, spmm
 from ..manager.graphEngine import RowRange
 from .op_util import halo_exchange, msg_all2all_GLOO
 
@@ -35,10 +36,11 @@ def _split(graph, feats: Tensor, x_halo: Tensor = None):
     return g, feats, x_halo
 
 
-def _run(g, x_local, x_halo, pre, post, mean, add_self, lo, hi, out=None, part=None, live=None):
+def _run(g, x_local, x_halo, pre, post, mean, add_self, lo, hi, out=None, part=None, live=None, rows=None):
     if isinstance(g, LocalGraph):
         return spmm(g, x_local, x_halo, pre, post, mean=mean, add_self=add_self, row_begin=lo, row_end=hi, out=out,
-                    part=part, live=live)
+                    part=part, live=live, rows=rows)
+    assert rows is None, "row lists are a device-path feature"
     from ..manager.graph_cpu import spmm_cpu          # gloo plumbing mode
     res = spmm_cpu(g, x_local, x_halo, pre, post, mean=mean, add_self=add_self, row_begin=lo, row_end=hi)
     if out is not None:
@@ -48,10 +50,12 @@ def _run(g, x_local, x_halo, pre, post, mean, add_self, lo, hi, out=None, part=N
 
 
 def GCN_aggregation(graph, feats: Tensor, mode: ProprogationMode = ProprogationMode.Forward,
-                    x_halo: Tensor = None, out: Tensor = None, part: str = None, live: Tensor = None) -> Tensor:
+                    x_halo: Tensor = None, out: Tensor = None, part: str = None, live: Tensor = None,
+                    rows: RowList = None) -> Tensor:
     """out[v] = norm2[v] * sum_{u->v} norm1[u] x[u] with global-degree norms (ops.py:17-32).
     `feats` may be cat(local, halo) as in the reference, or the local rows with `x_halo`.  `live`: row liveness
-    of the local rows (graph.row_live), so the gather skips the all-zero ones; the result is the same."""
+    of the local rows (graph.row_live), so the gather skips the all-zero ones; the result is the same.  `rows`:
+    only these destination rows of `out` are computed (graph.RowList), the others are left untouched."""
     g, x_local, x_halo = _split(graph, feats, x_halo)
     lo, hi = (graph.begin, graph.end) if isinstance(graph, RowRange) else (0, g.n_inner)
     if mode == ProprogationMode.Forward:
@@ -60,37 +64,37 @@ def GCN_aggregation(graph, feats: Tensor, mode: ProprogationMode = ProprogationM
         pre, post = g.norm["in_-0.5"], g.norm["out_-0.5"]
     else:
         raise ValueError(f"Invalid mode {mode}")
-    return _run(g, x_local, x_halo, pre, post, False, False, lo, hi, out, part, live)
+    return _run(g, x_local, x_halo, pre, post, False, False, lo, hi, out, part, live, rows)
 
 
 def SAGE_aggregation(graph, feats: Tensor, mode: ProprogationMode = ProprogationMode.Forward,
                      aggregator_type="mean", x_halo: Tensor = None, out: Tensor = None, part: str = None,
-                     live: Tensor = None) -> Tensor:
+                     live: Tensor = None, rows: RowList = None) -> Tensor:
     """ops.py:34-67: 'mean' = mean over in-neighbours (fwd) / sum of x[u]/outdeg[u] (bwd);
     'gcn' = (sum + self) / (indeg + 1) (fwd) / sum + self of x/(outdeg+1) (bwd)."""
     g, x_local, x_halo = _split(graph, feats, x_halo)
     lo, hi = (graph.begin, graph.end) if isinstance(graph, RowRange) else (0, g.n_inner)
     if mode == ProprogationMode.Forward:
         if aggregator_type == "mean":
-            return _run(g, x_local, x_halo, None, None, True, False, lo, hi, out, part, live)
+            return _run(g, x_local, x_halo, None, None, True, False, lo, hi, out, part, live, rows)
         if aggregator_type == "gcn":
-            return _run(g, x_local, x_halo, None, g.norm["in_+1_-1"], False, True, lo, hi, out, part, live)
+            return _run(g, x_local, x_halo, None, g.norm["in_+1_-1"], False, True, lo, hi, out, part, live, rows)
     elif mode == ProprogationMode.Backward:
         if aggregator_type == "mean":
-            return _run(g, x_local, x_halo, g.norm["out_-1"], None, False, False, lo, hi, out, part, live)
+            return _run(g, x_local, x_halo, g.norm["out_-1"], None, False, False, lo, hi, out, part, live, rows)
         if aggregator_type == "gcn":
-            return _run(g, x_local, x_halo, g.norm["out_+1_-1"], None, False, True, lo, hi, out, part, live)
+            return _run(g, x_local, x_halo, g.norm["out_+1_-1"], None, False, True, lo, hi, out, part, live, rows)
     else:
         raise ValueError(f"Invalid mode {mode}")
     raise ValueError(f"Invalid aggregator_type {aggregator_type}")
 
 
-def _aggregate(class_name: str, graph, x_local, x_halo, mode, out, part=None, live=None):
+def _aggregate(class_name: str, graph, x_local, x_halo, mode, out, part=None, live=None, rows=None):
     if class_name == "DistAggConv":
-        return GCN_aggregation(graph, x_local, mode=mode, x_halo=x_halo, out=out, part=part, live=live)
+        return GCN_aggregation(graph, x_local, mode=mode, x_halo=x_halo, out=out, part=part, live=live, rows=rows)
     if class_name == "DistAggSAGE":
         return SAGE_aggregation(graph, x_local, mode=mode, aggregator_type=engine.ctx.agg_type, x_halo=x_halo, out=out,
-                                part=part, live=live)
+                                part=part, live=live, rows=rows)
     raise ValueError(f"Invalid class_name {class_name}")
 
 
@@ -190,6 +194,46 @@ def _live_rows(local_messages: Tensor, layer: int, mode: ProprogationMode):
     return row_live(local_messages)
 
 
+# the rows the loss reads while train_for_one_epoch runs its forward pass (loss_rows); None outside it
+_LOSS_MASK: Optional[Tensor] = None
+
+
+@contextlib.contextmanager
+def loss_rows(mask: Tensor):
+    """Within this context the output layer's forward aggregation of a training pass computes only the rows `mask`
+    selects (a bool mask over the inner rows or their indices) and leaves the other rows zero.  That layer is
+    aggregate -> linear, so every other output row depends only on its own aggregated row: the rows the loss reads
+    come out bitwise the same.  train_for_one_epoch wraps its forward call in it; a model called directly still
+    computes every row."""
+    global _LOSS_MASK
+    prev = _LOSS_MASK
+    _LOSS_MASK = mask
+    try:
+        yield
+    finally:
+        _LOSS_MASK = prev
+
+
+def _loss_row_list(local_messages: Tensor, layer: int, is_train: bool,
+                   mode: ProprogationMode) -> Optional[Tuple[RowList, Optional[RowList], Optional[RowList]]]:
+    """(all, central, marginal) RowLists of the loss's rows when this aggregation is the output layer's training
+    forward on the device path inside loss_rows(), else None (central / marginal: the rows below / from
+    num_central, None without the decomposition).  Built once per mask (keyed on the mask object, its version and
+    the row split) and kept on the engine, so the launches never read a list that has been freed."""
+    mask, eng = _LOSS_MASK, engine.ctx
+    if (mask is None or not is_train or mode != ProprogationMode.Forward or layer != getattr(eng, "top_layer", None)
+            or not local_messages.is_cuda or comm.ctx.transport != "p2p"):
+        return None
+    key = (mask._version, eng.num_inner, eng.num_central if eng.use_parallel else None, local_messages.device)
+    cache = getattr(eng, "_loss_rows_cache", None)
+    if cache is None or cache[0] is not mask or cache[1] != key:
+        rows = row_list(mask, eng.num_inner, local_messages.device)
+        split = eng.num_central if eng.use_parallel else None
+        views = (rows, rows.below(split), rows.from_(split)) if split is not None else (rows, None, None)
+        eng._loss_rows_cache = cache = (mask, key, views)
+    return cache[2]
+
+
 def _finish(ctx, out: Tensor, layer: int, mode: ProprogationMode):
     if mode == ProprogationMode.Forward:
         ctx.saved = layer
@@ -209,8 +253,15 @@ def full_graph_propagation(ctx, local_messages: Tensor, graph, layer: int, is_tr
         with timer.record_events(f"{name}_quantization" if quant else f"{name}_communication"):
             pend = halo_exchange(local_messages, name, is_train)
         with timer.record_events(f"{name}_full_aggregation"):
-            live = _live_rows(local_messages, layer, mode)
-            out = _aggregate(class_name, g, local_messages, pend.halo, mode, None, live=live)
+            listed = _loss_row_list(local_messages, layer, is_train, mode)
+            if listed is not None:
+                # only the loss's rows; the rest stay zero (loss_rows)
+                out = local_messages.new_zeros((g.n_inner, local_messages.shape[1]))
+                if listed[0].n:
+                    _aggregate(class_name, g, local_messages, pend.halo, mode, out, rows=listed[0])
+            else:
+                live = _live_rows(local_messages, layer, mode)
+                out = _aggregate(class_name, g, local_messages, pend.halo, mode, None, live=live)
         pend.release()
     else:
         send_messages = local_messages[engine.ctx.total_send_idx]
@@ -250,31 +301,45 @@ def decomposed_graph_propagation(ctx, local_messages: Tensor, graph, layer: int,
         pend = halo_exchange(local_messages, name, is_train, stream=side)
     landed = torch.cuda.Event(enable_timing=True)
     landed.record(side)
-    out = local_messages.new_empty((eng.num_inner, local_messages.shape[1]))
+    listed = _loss_row_list(local_messages, layer, is_train, mode)
+    # with a row list (loss_rows) each launch gets the list's rows of its range, an empty one is skipped, and the
+    # rows nobody lists stay zero
+    _, central_rows, marginal_rows = listed if listed is not None else (None, None, None)
+    run_central = listed is None or central_rows.n > 0
+    run_marginal = listed is None or marginal_rows.n > 0
+    if listed is None:
+        out = local_messages.new_empty((eng.num_inner, local_messages.shape[1]))
     with timer.record_events(f"{name}_central_aggregation"):
+        if listed is not None:
+            out = local_messages.new_zeros((eng.num_inner, local_messages.shape[1]))
         live = _live_rows(local_messages, layer, mode)
-        _aggregate(class_name, graph.central_graph, local_messages, None, mode, out[:eng.num_central], live=live)
+        if run_central:
+            _aggregate(class_name, graph.central_graph, local_messages, None, mode, out[:eng.num_central], live=live,
+                       rows=central_rows)
     if _split_marginal():
         # the marginal rows' LOCAL-source neighbours do not need the halo either: aggregate them while
         # the exchange is still in flight; only the halo-source segment of each row waits for it
         with timer.record_events(f"{name}_marginal_aggregation_local"):
-            _aggregate(class_name, graph.marginal_graph, local_messages, None, mode, out[eng.num_central:],
-                       part="local", live=live)
+            if run_marginal:
+                _aggregate(class_name, graph.marginal_graph, local_messages, None, mode, out[eng.num_central:],
+                           part="local", live=live, rows=marginal_rows)
         overlappable_done = torch.cuda.Event(enable_timing=True)
         overlappable_done.record(main)
         timer.record_exposed(name, overlappable_done, landed)
         main.wait_event(landed)
         with timer.record_events(f"{name}_marginal_aggregation_halo"):
-            _aggregate(class_name, graph.marginal_graph, local_messages, pend.halo, mode, out[eng.num_central:],
-                       part="halo", live=live)
+            if run_marginal:
+                _aggregate(class_name, graph.marginal_graph, local_messages, pend.halo, mode, out[eng.num_central:],
+                           part="halo", live=live, rows=marginal_rows)
     else:
         central_done = torch.cuda.Event(enable_timing=True)
         central_done.record(main)
         timer.record_exposed(name, central_done, landed)
         main.wait_event(landed)
         with timer.record_events(f"{name}_marginal_aggregation"):
-            _aggregate(class_name, graph.marginal_graph, local_messages, pend.halo, mode, out[eng.num_central:],
-                       live=live)
+            if run_marginal:
+                _aggregate(class_name, graph.marginal_graph, local_messages, pend.halo, mode, out[eng.num_central:],
+                           live=live, rows=marginal_rows)
     pend.release()
     local_messages.record_stream(side)
     return _finish(ctx, out, layer, mode)

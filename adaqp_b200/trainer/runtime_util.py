@@ -22,6 +22,7 @@ from ..assigner import Assigner as assigner
 from ..communicator import Communicator as comm
 from ..helper import BitType
 from ..manager import GraphEngine as engine
+from ..model import ops
 
 _nccl_group = None
 
@@ -118,7 +119,9 @@ def train_for_one_epoch(epoch: int, graph, model: nn.Module, input_data: Tensor,
             overhead = time.time() - t0
     epoch_start = time.time()
     model.train()
-    logits = model(graph, input_data)
+    # the loss reads only the train rows: the output layer's aggregation computes just those (ops.loss_rows)
+    with ops.loss_rows(train_mask):
+        logits = model(graph, input_data)
     loss = criterion(logits[train_mask], labels[train_mask]) / total_num_training_samples
     optimizer.zero_grad()
     loss.backward()

@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define ADAQP_ABI_VERSION 7
+#define ADAQP_ABI_VERSION 8
 
 #define ADAQP_EINVAL (-1)   /* bad argument (bits not in {1,2,4,8}, negative size ...) */
 #define ADAQP_EALIGN (-2)   /* pointer alignment requirement violated */
@@ -232,13 +232,19 @@ int adaqp_spmm_csr_f32(const int64_t *indptr, const int32_t *indices,
  * `live` (NULL = every source row is read): uint8 per local source row, 0 where the row of x0 is all
  * zeros (adaqp_row_live_f32).  The gather then skips the neighbours u < n_split with live[u] == 0 and a
  * finite pre[u]; they add exactly zero, so the result is the same (DESIGN §3).  Halo sources are always
- * read.  The opt-in spmm_impl variants 2-4 ignore `live`. */
+ * read.  The opt-in spmm_impl variants 2-4 ignore `live`.
+ * `rows` (NULL = every row of [row_begin, row_end)): a device list of n_list int32 destination row ids,
+ * absolute CSR ids inside [row_begin, row_end), ascending and unique.  Only those rows are computed, each
+ * exactly as without the list, into out + (row - row_begin) * ldo; the other output rows are neither read
+ * nor written.  0 <= n_list <= row_end - row_begin (ADAQP_EINVAL otherwise); n_list == 0 launches nothing.
+ * The ids themselves are the caller's to check (they live on the device).  `rows` and `live` cannot be
+ * combined, and a list always takes the default kernels (spmm_impl 2-4 are not used with it). */
 int adaqp_spmm_csr_seg_f32(const int64_t *indptr, const int64_t *seg_start, const int64_t *seg_end,
                            const int32_t *indices, const float *x0, int64_t ld0, int64_t n_split,
                            const float *x1, int64_t ld1, const float *pre, const float *post,
                            int mean, int add_self, int accumulate, int64_t row_begin,
                            int64_t row_end, int32_t F, float *out, int64_t ldo, const uint8_t *live,
-                           void *stream);
+                           const int32_t *rows, int64_t n_list, void *stream);
 
 /* live[r] = 1 if some x[r, c] != 0 (a NaN counts as nonzero), else 0, for r < rows; x is [rows, F] fp32 with
  * pitch ld.  One coalesced read of x on `stream`. */
