@@ -97,6 +97,20 @@ def row_list(mask: torch.Tensor, n_rows: int, device) -> RowList:
     return RowList(torch.from_numpy(host).to(device), host)
 
 
+def part_segments(graph: LocalGraph, part: Optional[str]):
+    """(seg_start, seg_end, accumulate) of one launch over CSR rows, by how the launch splits each row for the
+    two-pass marginal schedule: part=None reads whole rows; 'local' reads each row's local-source segment only (up to
+    halo_split), which needs no halo; 'halo' reads its halo-source segment (from halo_split) and accumulates into
+    what the local part wrote."""
+    if part is None:
+        return None, None, 0
+    if part == "local":
+        return None, graph.halo_split.data_ptr(), 0
+    if part == "halo":
+        return graph.halo_split.data_ptr(), None, 1
+    raise ValueError(part)
+
+
 def spmm(graph: LocalGraph, x_local: torch.Tensor, x_halo: Optional[torch.Tensor],
          pre: Optional[torch.Tensor], post: Optional[torch.Tensor], mean: bool = False,
          add_self: bool = False, row_begin: int = 0, row_end: Optional[int] = None,
@@ -125,16 +139,10 @@ def spmm(graph: LocalGraph, x_local: torch.Tensor, x_halo: Optional[torch.Tensor
         n_list = rows.n
     if x_halo is not None and x_halo.shape[0] == 0:
         x_halo = None
-    seg_start = seg_end = None
-    accumulate = 0
-    if part == "local":
-        seg_end = graph.halo_split.data_ptr()
-    elif part == "halo":
+    seg_start, seg_end, accumulate = part_segments(graph, part)
+    if part == "halo":
         assert out is not None, "the halo part accumulates into the output of the local part"
-        seg_start = graph.halo_split.data_ptr()
-        accumulate, add_self = 1, False
-    elif part is not None:
-        raise ValueError(part)
+        add_self = False
     if live is not None:
         assert live.dtype == torch.uint8 and live.is_contiguous() and live.numel() >= graph.n_inner
     rc = L.adaqp_spmm_csr_seg_f32(
@@ -188,15 +196,7 @@ def appnp_prop(graph: LocalGraph, x_local: torch.Tensor, x_halo: Optional[torch.
         out = torch.empty((row_end - row_begin, F), dtype=torch.float32, device=x_local.device)
     if x_halo is not None and x_halo.shape[0] == 0:
         x_halo = None
-    seg_start = seg_end = None
-    accumulate = 0
-    if part == "local":
-        seg_end = graph.halo_split.data_ptr()
-    elif part == "halo":
-        seg_start = graph.halo_split.data_ptr()
-        accumulate = 1
-    elif part is not None:
-        raise ValueError(part)
+    seg_start, seg_end, accumulate = part_segments(graph, part)
     for t in (tele, acc):
         assert t is None or (t.dtype == torch.float32 and t.stride(1) == 1 and t.shape[0] >= row_end - row_begin)
     rc = L.adaqp_appnp_prop_f32(

@@ -241,28 +241,116 @@ def _finish(ctx, out: Tensor, layer: int, mode: ProprogationMode):
     return out, None, None, None
 
 
+def _full(graph) -> LocalGraph:
+    """The whole LocalGraph of a graph argument (a DecompGraph in the overlapped mode)."""
+    return graph.full if isinstance(graph, DecompGraph) else graph
+
+
+def _p2p_only(model: str):
+    if comm.ctx.transport != "p2p":
+        raise NotImplementedError(f"{model} runs on the p2p transport only (not the CPU gloo plumbing mode)")
+
+
+def _comm_name(name: str, is_train: bool) -> str:
+    """Timer region of an exchange on `name`: quantised in training under the QUANT precision."""
+    quant = engine.ctx.bit_type == BitType.QUANT and is_train
+    return f"{name}_quantization" if quant else f"{name}_communication"
+
+
+def _propagate(name: str, comm_name: str, exchange, aggregate, split: bool = False, sent: Tuple[Tensor, ...] = ()):
+    """The exchange-and-overlap schedule of every aggregation on the p2p transport.
+
+    exchange(stream) enqueues the exchange on `stream` (the current one when None) and returns (halo, aux, release);
+    aggregate(lo, hi, halo, aux, part=None) runs the kernel over inner rows [lo, hi) and the result of its last call
+    is returned; release() lets the senders reuse the received rows once their last consumer has been enqueued.
+    Without the overlap (engine.ctx.use_parallel off) the exchange and then every row run on the current stream.
+    With it the exchange runs on engine.ctx.marginal_stream while the central rows, which have no halo neighbour in
+    either direction (so halo and aux are None), run on the current stream; the marginal rows run in one pass once
+    the halo has landed, or, with `split` (a kernel whose local and halo sources combine exactly) and
+    ADAQP_MARGINAL_SPLIT on, as part='local' while the exchange is in flight and part='halo' after it.  `sent` are
+    the tensors the side stream reads."""
+    eng, timer = engine.ctx, engine.ctx.timer
+    if not eng.use_parallel:
+        with timer.record_events(comm_name):
+            halo, aux, release = exchange(None)
+        with timer.record_events(f"{name}_full_aggregation"):
+            kept = aggregate(0, eng.num_inner, halo, aux)
+        release()
+        return kept
+    main, side = torch.cuda.current_stream(), eng.marginal_stream
+    ready = torch.cuda.Event()
+    ready.record(main)                       # what is sent is produced on the default stream
+    side.wait_event(ready)
+    with timer.record_events(comm_name, stream=side):
+        halo, aux, release = exchange(side)
+    landed = torch.cuda.Event(enable_timing=True)
+    landed.record(side)
+    nc, n = eng.num_central, eng.num_inner
+    with timer.record_events(f"{name}_central_aggregation"):
+        aggregate(0, nc, None, None)
+    region, part = f"{name}_marginal_aggregation", None
+    if split and _split_marginal():
+        # the marginal rows' local-source neighbours do not need the halo either: aggregate them while the exchange
+        # is still in flight; only the halo-source segment of each row waits for it
+        with timer.record_events(f"{region}_local"):
+            aggregate(nc, n, None, None, part="local")
+        region, part = f"{region}_halo", "halo"
+    overlappable_done = torch.cuda.Event(enable_timing=True)
+    overlappable_done.record(main)
+    timer.record_exposed(name, overlappable_done, landed)
+    main.wait_event(landed)
+    with timer.record_events(region):
+        kept = aggregate(nc, n, halo, aux, part=part)
+    release()
+    for t in sent:
+        t.record_stream(side)
+    return kept
+
+
+def _p2p_propagation(name: str, local_messages: Tensor, graph, layer: int, is_train: bool, mode: ProprogationMode,
+                     class_name: str) -> Tensor:
+    """The p2p transport of full_graph_propagation / decomposed_graph_propagation: _propagate over the halo exchange
+    of local_messages.  The output layer's backward pass skips the all-zero gradient rows (_live_rows); its training
+    forward inside loss_rows() computes only the loss's rows, each launch the list's rows of its range, and leaves
+    the other rows zero.  Both are set up inside the first aggregation region (full, or central)."""
+    eng, g = engine.ctx, _full(graph)
+    listed = _loss_row_list(local_messages, layer, is_train, mode)
+    out = live = None
+
+    def exchange(stream):
+        pend = halo_exchange(local_messages, name, is_train, stream=stream)
+        return pend.halo, None, pend.release
+
+    def aggregate(lo, hi, halo, _, part=None):
+        nonlocal out, live
+        if out is None:
+            shape = (eng.num_inner, local_messages.shape[1])
+            if listed is None:
+                out, live = local_messages.new_empty(shape), _live_rows(local_messages, layer, mode)
+            else:
+                out = local_messages.new_zeros(shape)
+        rows = None
+        if listed is not None:
+            # the whole list, or its central / marginal share; an empty share launches nothing
+            rows = listed[0] if (lo, hi) == (0, eng.num_inner) else listed[1] if lo == 0 else listed[2]
+            if not rows.n:
+                return out
+        _aggregate(class_name, RowRange(g, lo, hi), local_messages, halo, mode, out[lo:hi], part=part, live=live,
+                   rows=rows)
+        return out
+
+    return _propagate(name, _comm_name(name, is_train), exchange, aggregate, split=True, sent=(local_messages,))
+
+
 def full_graph_propagation(ctx, local_messages: Tensor, graph, layer: int, is_train: bool,
                            mode: ProprogationMode, class_name: str):
     """Exchange, then aggregate every inner row (ops.py:132-154)."""
     name = f"forward{layer}" if mode == ProprogationMode.Forward else f"backward{layer}"
     local_messages = local_messages.contiguous()
     timer = engine.ctx.timer
-    g = graph.full if isinstance(graph, DecompGraph) else graph
+    g = _full(graph)
     if comm.ctx.transport == "p2p":
-        quant = engine.ctx.bit_type == BitType.QUANT and is_train
-        with timer.record_events(f"{name}_quantization" if quant else f"{name}_communication"):
-            pend = halo_exchange(local_messages, name, is_train)
-        with timer.record_events(f"{name}_full_aggregation"):
-            listed = _loss_row_list(local_messages, layer, is_train, mode)
-            if listed is not None:
-                # only the loss's rows; the rest stay zero (loss_rows)
-                out = local_messages.new_zeros((g.n_inner, local_messages.shape[1]))
-                if listed[0].n:
-                    _aggregate(class_name, g, local_messages, pend.halo, mode, out, rows=listed[0])
-            else:
-                live = _live_rows(local_messages, layer, mode)
-                out = _aggregate(class_name, g, local_messages, pend.halo, mode, None, live=live)
-        pend.release()
+        out = _p2p_propagation(name, local_messages, graph, layer, is_train, mode, class_name)
     else:
         send_messages = local_messages[engine.ctx.total_send_idx]
         remote = msg_all2all_GLOO(send_messages, name, is_train)
@@ -292,132 +380,34 @@ def decomposed_graph_propagation(ctx, local_messages: Tensor, graph, layer: int,
         with timer.record(f"{name}_marginal_aggregation"):
             _aggregate(class_name, graph.marginal_graph, local_messages, remote, mode, out[eng.num_central:])
         return _finish(ctx, out, layer, mode)
-    main, side = torch.cuda.current_stream(), eng.marginal_stream
-    quant = eng.bit_type == BitType.QUANT and is_train
-    ready = torch.cuda.Event()
-    ready.record(main)                       # local_messages is produced on the default stream
-    side.wait_event(ready)
-    with timer.record_events(f"{name}_quantization" if quant else f"{name}_communication", stream=side):
-        pend = halo_exchange(local_messages, name, is_train, stream=side)
-    landed = torch.cuda.Event(enable_timing=True)
-    landed.record(side)
-    listed = _loss_row_list(local_messages, layer, is_train, mode)
-    # with a row list (loss_rows) each launch gets the list's rows of its range, an empty one is skipped, and the
-    # rows nobody lists stay zero
-    _, central_rows, marginal_rows = listed if listed is not None else (None, None, None)
-    run_central = listed is None or central_rows.n > 0
-    run_marginal = listed is None or marginal_rows.n > 0
-    if listed is None:
-        out = local_messages.new_empty((eng.num_inner, local_messages.shape[1]))
-    with timer.record_events(f"{name}_central_aggregation"):
-        if listed is not None:
-            out = local_messages.new_zeros((eng.num_inner, local_messages.shape[1]))
-        live = _live_rows(local_messages, layer, mode)
-        if run_central:
-            _aggregate(class_name, graph.central_graph, local_messages, None, mode, out[:eng.num_central], live=live,
-                       rows=central_rows)
-    if _split_marginal():
-        # the marginal rows' LOCAL-source neighbours do not need the halo either: aggregate them while
-        # the exchange is still in flight; only the halo-source segment of each row waits for it
-        with timer.record_events(f"{name}_marginal_aggregation_local"):
-            if run_marginal:
-                _aggregate(class_name, graph.marginal_graph, local_messages, None, mode, out[eng.num_central:],
-                           part="local", live=live, rows=marginal_rows)
-        overlappable_done = torch.cuda.Event(enable_timing=True)
-        overlappable_done.record(main)
-        timer.record_exposed(name, overlappable_done, landed)
-        main.wait_event(landed)
-        with timer.record_events(f"{name}_marginal_aggregation_halo"):
-            if run_marginal:
-                _aggregate(class_name, graph.marginal_graph, local_messages, pend.halo, mode, out[eng.num_central:],
-                           part="halo", live=live, rows=marginal_rows)
-    else:
-        central_done = torch.cuda.Event(enable_timing=True)
-        central_done.record(main)
-        timer.record_exposed(name, central_done, landed)
-        main.wait_event(landed)
-        with timer.record_events(f"{name}_marginal_aggregation"):
-            if run_marginal:
-                _aggregate(class_name, graph.marginal_graph, local_messages, pend.halo, mode, out[eng.num_central:],
-                           live=live, rows=marginal_rows)
-    pend.release()
-    local_messages.record_stream(side)
-    return _finish(ctx, out, layer, mode)
+    return _finish(ctx, _p2p_propagation(name, local_messages, graph, layer, is_train, mode, class_name), layer, mode)
 
 
 # ---------------------------------------------------------------- GAT
 def _gat_exchange(rows: Tensor, name: str, is_train: bool, scalars: Tensor, aux_key: str, stream=None):
     """Exchange the boundary rows of one layer key (quantised per mode, as halo_exchange does for GCN / SAGE) and
     their per-row attention scalars in fp32 on `aux_key`: both ranks must compute the softmax from identical
-    scalars.  Returns (pending row exchange, received scalar rows [num_remote, width])."""
+    scalars.  Returns (halo rows, received scalar rows [num_remote, width], release), as _propagate's exchange."""
     ex = comm.ctx.comm_buffer.p2p
     ex.post_send_fp(aux_key, scalars, stream=stream)
     pend = halo_exchange(rows, name, is_train, stream=stream)
-    return pend, ex.complete_recv_fp(aux_key, stream=stream)
+    aux_halo = ex.complete_recv_fp(aux_key, stream=stream)
+
+    def release():
+        pend.release()
+        ex.release_fp(aux_key)
+    return pend.halo, aux_halo, release
 
 
-def _gat_release(pend, aux_key: str):
-    """After the last consumer of the received rows has been enqueued on the current stream."""
-    pend.release()
-    if aux_key is not None:
-        comm.ctx.comm_buffer.p2p.release_fp(aux_key)
-
-
-def _gat_propagate(name: str, quant: bool, rows: Tensor, scalars: Tensor, aux_key: str, is_train: bool, aggregate,
-                   split: bool = False):
-    """Exchange + aggregation skeleton of full_graph_propagation / decomposed_graph_propagation for the models with
-    their own kernels (GAT, SAGE max-pool): aggregate(lo, hi, halo_rows, halo_scalars) runs the kernel over inner
-    rows [lo, hi).  `scalars` (None: rows only) travel in fp32 on `aux_key`.  Central rows have no halo neighbour in
-    either direction, so in the overlapped mode they run while the exchange is in flight.  The marginal rows run in
-    one pass once it has landed, or, with `split` (a kernel whose local and halo sources combine exactly) and
-    ADAQP_MARGINAL_SPLIT on, as aggregate(..., part='local') in flight and aggregate(..., part='halo') after."""
-    eng, timer = engine.ctx, engine.ctx.timer
-    comm_name = f"{name}_quantization" if quant else f"{name}_communication"
-
-    def exchange(stream=None):
-        if scalars is None:
-            return halo_exchange(rows, name, is_train, stream=stream), None
-        return _gat_exchange(rows, name, is_train, scalars, aux_key, stream=stream)
-
-    if not eng.use_parallel:
-        with timer.record_events(comm_name):
-            pend, aux_halo = exchange()
-        with timer.record_events(f"{name}_full_aggregation"):
-            kept = aggregate(0, eng.num_inner, pend.halo, aux_halo)
-        _gat_release(pend, aux_key)
-        return kept
-    main, side = torch.cuda.current_stream(), eng.marginal_stream
-    ready = torch.cuda.Event()
-    ready.record(main)                       # rows and scalars are produced on the default stream
-    side.wait_event(ready)
-    with timer.record_events(comm_name, stream=side):
-        pend, aux_halo = exchange(stream=side)
-    landed = torch.cuda.Event(enable_timing=True)
-    landed.record(side)
-    nc = eng.num_central
-    with timer.record_events(f"{name}_central_aggregation"):
-        aggregate(0, nc, None, None)
-    if split and _split_marginal():
-        with timer.record_events(f"{name}_marginal_aggregation_local"):
-            aggregate(nc, eng.num_inner, None, None, part="local")
-        overlappable_done = torch.cuda.Event(enable_timing=True)
-        overlappable_done.record(main)
-        timer.record_exposed(name, overlappable_done, landed)
-        main.wait_event(landed)
-        with timer.record_events(f"{name}_marginal_aggregation_halo"):
-            kept = aggregate(nc, eng.num_inner, pend.halo, aux_halo, part="halo")
-    else:
-        central_done = torch.cuda.Event(enable_timing=True)
-        central_done.record(main)
-        timer.record_exposed(name, central_done, landed)
-        main.wait_event(landed)
-        with timer.record_events(f"{name}_marginal_aggregation"):
-            kept = aggregate(nc, eng.num_inner, pend.halo, aux_halo)
-    _gat_release(pend, aux_key)
-    rows.record_stream(side)
-    if scalars is not None:
-        scalars.record_stream(side)
-    return kept
+def _exchange(rows: Tensor, name: str, is_train: bool, scalars: Tensor = None, aux_key: str = None):
+    """_propagate's exchange for the models with their own kernels: `rows` on `name`, and with `scalars` their
+    per-row scalars in fp32 on `aux_key` (_gat_exchange)."""
+    def exchange(stream):
+        if scalars is not None:
+            return _gat_exchange(rows, name, is_train, scalars, aux_key, stream=stream)
+        pend = halo_exchange(rows, name, is_train, stream=stream)
+        return pend.halo, None, pend.release
+    return exchange
 
 
 class DistAggGAT(Function):
@@ -432,25 +422,24 @@ class DistAggGAT(Function):
 
     @staticmethod
     def forward(ctx, z: Tensor, a_l: Tensor, a_r: Tensor, graph, layer: int, is_train: bool, heads: int) -> Tensor:
-        if comm.ctx.transport != "p2p":
-            raise NotImplementedError("GAT runs on the p2p transport only (not the CPU gloo plumbing mode)")
-        eng = engine.ctx
+        _p2p_only("GAT")
         z = z.contiguous()
         n, F = z.shape
         el, er = gat.scores(z, a_l, a_r, heads)
-        g = graph.full if isinstance(graph, DecompGraph) else graph
+        g = _full(graph)
         out = z.new_empty((n, F))
         lse = z.new_empty((n, heads))
         fwd_key, _ = attn_keys(layer)
+        name = f"forward{layer}"
 
-        def aggregate(lo, hi, z_halo, el_halo):
+        def aggregate(lo, hi, z_halo, el_halo, part=None):
             if z_halo is not None and is_train:          # kept for the backward pass; the slab rows are reused
                 z_halo, el_halo = z_halo.clone(), el_halo.clone()
             gat.forward(g, z, z_halo, el, el_halo, er, heads, lo, hi, out[lo:hi], lse[lo:hi])
             return z_halo, el_halo
 
-        quant = eng.bit_type == BitType.QUANT and is_train
-        z_halo, el_halo = _gat_propagate(f"forward{layer}", quant, z, el, fwd_key, is_train, aggregate)
+        z_halo, el_halo = _propagate(name, _comm_name(name, is_train), _exchange(z, name, is_train, el, fwd_key),
+                                     aggregate, sent=(z, el))
         if is_train:
             ctx.save_for_backward(z, z_halo, el, el_halo, er, out, lse, a_l, a_r)
             ctx.graph, ctx.layer, ctx.heads = graph, layer, heads
@@ -465,19 +454,20 @@ class DistAggGAT(Function):
         D = F // heads
         s = (grad.view(n, heads, D) * out.view(n, heads, D)).sum(-1)
         aux = torch.cat([er, lse, s], 1).contiguous()
-        g = ctx.graph.full if isinstance(ctx.graph, DecompGraph) else ctx.graph
+        g = _full(ctx.graph)
         dz = z.new_empty((n, F))
         dl = z.new_empty((n, heads))
         dr = z.new_empty((n, heads))
         _, bwd_key = attn_keys(layer)
+        name = f"backward{layer}"
 
-        def aggregate(lo, hi, g_halo, aux_halo):
+        def aggregate(lo, hi, g_halo, aux_halo, part=None):
             halo = (g_halo, z_halo, el_halo, aux_halo) if g_halo is not None else (None,) * 4
             gat.backward(g, grad, halo[0], z, halo[1], el, halo[2], aux, halo[3], a_l, a_r, heads, lo, hi,
                          dz[lo:hi], dl[lo:hi], dr[lo:hi])
 
-        quant = engine.ctx.bit_type == BitType.QUANT
-        _gat_propagate(f"backward{layer}", quant, grad, aux, bwd_key, True, aggregate)
+        _propagate(name, _comm_name(name, True), _exchange(grad, name, True, aux, bwd_key), aggregate,
+                   sent=(grad, aux))
         zh = z.view(n, heads, D)
         da_l = (dl.unsqueeze(-1) * zh).sum(0)
         da_r = (dr.unsqueeze(-1) * zh).sum(0)
@@ -501,23 +491,21 @@ class DistAggGATv2(Function):
 
     @staticmethod
     def forward(ctx, zs: Tensor, zd: Tensor, attn: Tensor, graph, layer: int, is_train: bool, heads: int) -> Tensor:
-        if comm.ctx.transport != "p2p":
-            raise NotImplementedError("GATv2 runs on the p2p transport only (not the CPU gloo plumbing mode)")
-        eng = engine.ctx
+        _p2p_only("GATv2")
         zs, zd = zs.contiguous(), zd.contiguous()
         n, F = zs.shape
-        g = graph.full if isinstance(graph, DecompGraph) else graph
+        g = _full(graph)
         out = zs.new_empty((n, F))
         lse = zs.new_empty((n, heads))
+        name = f"forward{layer}"
 
-        def aggregate(lo, hi, zs_halo, _):
+        def aggregate(lo, hi, zs_halo, _, part=None):
             if zs_halo is not None and is_train:          # kept for the backward pass; the slab rows are reused
                 zs_halo = zs_halo.clone()
             gatv2.forward(g, zs, zs_halo, zd, attn, heads, lo, hi, out[lo:hi], lse[lo:hi])
             return zs_halo
 
-        quant = eng.bit_type == BitType.QUANT and is_train
-        zs_halo = _gat_propagate(f"forward{layer}", quant, zs, None, None, is_train, aggregate)
+        zs_halo = _propagate(name, _comm_name(name, is_train), _exchange(zs, name, is_train), aggregate, sent=(zs,))
         if is_train:
             if zs_halo is None:
                 zs_halo = zs.new_empty((0, F))
@@ -532,8 +520,8 @@ class DistAggGATv2(Function):
         heads, layer = ctx.heads, ctx.layer
         n, F = zs.shape
         D = F // heads
-        eng, timer, ex = engine.ctx, engine.ctx.timer, comm.ctx.comm_buffer.p2p
-        g = ctx.graph.full if isinstance(ctx.graph, DecompGraph) else ctx.graph
+        eng, ex = engine.ctx, comm.ctx.comm_buffer.p2p
+        g = _full(ctx.graph)
         S = (grad.view(n, heads, D) * out.view(n, heads, D)).sum(-1).contiguous()
         halo_indptr, halo_dst = eng.gatv2_halo
         fold = eng.gatv2_fold
@@ -541,38 +529,17 @@ class DistAggGATv2(Function):
         dzs_halo = gatv2.backward_halo(halo_indptr, halo_dst, zs_halo, zd, grad, lse, S, attn, heads)
         dzs, dzd, da = (zs.new_empty((n, F)) for _ in range(3))
 
-        def inner(lo, hi, push):
+        def exchange(stream):
+            ex.post_send_fp(key, dzs_halo, stream=stream)
+            return ex.complete_recv_fp(key, stream=stream), None, lambda: ex.release_fp(key)
+
+        def aggregate(lo, hi, push, _, part=None):
+            # central rows are sent to no peer, so nothing is pushed to them (push is None)
             gatv2.backward_inner(g, zs, zs_halo, zd, grad, lse, S, attn, heads, push, fold if push is not None else None,
                                  lo, hi, dzs[lo:hi], dzd[lo:hi], da[lo:hi])
 
-        if not eng.use_parallel:
-            with timer.record_events(f"{name}_communication"):
-                ex.post_send_fp(key, dzs_halo)
-                push = ex.complete_recv_fp(key)
-            with timer.record_events(f"{name}_full_aggregation"):
-                inner(0, n, push)
-            ex.release_fp(key)
-        else:
-            main, side = torch.cuda.current_stream(), eng.marginal_stream
-            ready = torch.cuda.Event()
-            ready.record(main)                   # dzs_halo is produced on the default stream
-            side.wait_event(ready)
-            with timer.record_events(f"{name}_communication", stream=side):
-                ex.post_send_fp(key, dzs_halo, stream=side)
-                push = ex.complete_recv_fp(key, stream=side)
-            landed = torch.cuda.Event(enable_timing=True)
-            landed.record(side)
-            nc = eng.num_central
-            with timer.record_events(f"{name}_central_aggregation"):
-                inner(0, nc, None)               # central rows are sent to no peer, so nothing is pushed to them
-            central_done = torch.cuda.Event(enable_timing=True)
-            central_done.record(main)
-            timer.record_exposed(name, central_done, landed)
-            main.wait_event(landed)
-            with timer.record_events(f"{name}_marginal_aggregation"):
-                inner(nc, n, push)
-            ex.release_fp(key)
-            dzs_halo.record_stream(side)
+        # the push is fp32 in every mode
+        _propagate(name, f"{name}_communication", exchange, aggregate, sent=(dzs_halo,))
         return dzs, dzd, da.sum(0).view_as(attn), None, None, None, None
 
 
@@ -591,20 +558,18 @@ class DistAggSAGEPool(Function):
 
     @staticmethod
     def forward(ctx, p: Tensor, graph, layer: int, is_train: bool) -> Tensor:
-        if comm.ctx.transport != "p2p":
-            raise NotImplementedError("SAGE max-pool runs on the p2p transport only (not the CPU gloo plumbing mode)")
-        eng = engine.ctx
+        _p2p_only("SAGE max-pool")
         p = p.contiguous()
         n, F = p.shape
-        g = graph.full if isinstance(graph, DecompGraph) else graph
+        g = _full(graph)
         m = p.new_empty((n, F))
         arg = torch.empty((n, F), dtype=torch.int32, device=p.device)
+        name = f"forward{layer}"
 
         def aggregate(lo, hi, p_halo, _, part=None):
             sage_pool.forward(g, p, p_halo, lo, hi, m[lo:hi], arg[lo:hi], part=part)
 
-        quant = eng.bit_type == BitType.QUANT and is_train
-        _gat_propagate(f"forward{layer}", quant, p, None, None, is_train, aggregate, split=True)
+        _propagate(name, _comm_name(name, is_train), _exchange(p, name, is_train), aggregate, split=True, sent=(p,))
         if is_train:
             ctx.save_for_backward(arg)
             ctx.graph, ctx.layer = graph, layer
@@ -614,35 +579,35 @@ class DistAggSAGEPool(Function):
     def backward(ctx: Any, *grad_outputs: Tuple[Tensor, ...]):
         arg, = ctx.saved_tensors
         grad = grad_outputs[0].contiguous()
-        g = ctx.graph.full if isinstance(ctx.graph, DecompGraph) else ctx.graph
+        g = _full(ctx.graph)
         want = engine.ctx.pool_want
         dp = grad.new_empty(grad.shape)
+        arg_rows, name = arg.view(torch.float32), f"backward{ctx.layer}"
 
         def aggregate(lo, hi, g_halo, arg_halo, part=None):
             a_halo = arg_halo.view(torch.int32) if arg_halo is not None else None
             sage_pool.backward(g, want, grad, g_halo, arg, a_halo, lo, hi, dp[lo:hi], part=part)
 
-        quant = engine.ctx.bit_type == BitType.QUANT
-        _gat_propagate(f"backward{ctx.layer}", quant, grad, arg.view(torch.float32), pool_arg_key(ctx.layer), True,
-                       aggregate, split=True)
+        _propagate(name, _comm_name(name, True), _exchange(grad, name, True, arg_rows, pool_arg_key(ctx.layer)),
+                   aggregate, split=True, sent=(grad, arg_rows))
         return dp, None, None, None
 
 
 # ---------------------------------------------------------------- APPNP / GCNII propagation steps
-def _teleport_step(name: str, quant: bool, g: LocalGraph, h: Tensor, z: Tensor, alpha: float, is_train: bool) -> Tensor:
+def _teleport_step(name: str, g: LocalGraph, h: Tensor, z: Tensor, alpha: float, is_train: bool) -> Tensor:
     """out = (1 - alpha) A h + alpha z over the exchange of h on `name` (A with the GCN forward norms): one
-    appnp_prop launch per row range of _gat_propagate's overlap, the teleport term in the kernel's epilogue."""
+    appnp_prop launch per row range of _propagate's overlap, the teleport term in the kernel's epilogue."""
     pre, post = g.norm["out_-0.5"], g.norm["in_-0.5"]
     out = torch.empty_like(z)
 
     def aggregate(lo, hi, h_halo, _, part=None):
         appnp_prop(g, h, h_halo, pre, post, 1.0 - alpha, alpha, lo, hi, out[lo:hi], tele=z[lo:hi], part=part)
 
-    _gat_propagate(name, quant, h, None, None, is_train, aggregate, split=True)
+    _propagate(name, _comm_name(name, is_train), _exchange(h, name, is_train), aggregate, split=True, sent=(h,))
     return out
 
 
-def _accum_step(name: str, quant: bool, g: LocalGraph, grad: Tensor, acc: Tensor, alpha: float, mode: int) -> Tensor:
+def _accum_step(name: str, g: LocalGraph, grad: Tensor, acc: Tensor, alpha: float, mode: int) -> Tensor:
     """out = (1 - alpha) A^T grad over the exchange of grad on `name` (the swapped norms), and in the same pass the
     acc term alpha * grad of each row, stored into / added to `acc` or folded into out per `mode` (ACC_* bits)."""
     pre, post = g.norm["in_-0.5"], g.norm["out_-0.5"]
@@ -652,7 +617,7 @@ def _accum_step(name: str, quant: bool, g: LocalGraph, grad: Tensor, acc: Tensor
         appnp_prop(g, grad, g_halo, pre, post, 1.0 - alpha, alpha, lo, hi, out[lo:hi], acc=acc[lo:hi], acc_mode=mode,
                    part=part)
 
-    _gat_propagate(name, quant, grad, None, None, True, aggregate, split=True)
+    _propagate(name, _comm_name(name, True), _exchange(grad, name, True), aggregate, split=True, sent=(grad,))
     return out
 
 
@@ -666,20 +631,17 @@ class DistAPPNPProp(Function):
     g_k = (1 - alpha) A^T g_{k+1} exchanges g_{k+1} on backward{k} (k = K-1 .. 0), the kernel also accumulates
     alpha g_{k+1} of each row, and the last step writes dz = alpha sum_{k=1..K} g_k + g_0 directly.  Quantisation is
     the identity in backward (straight-through), as in DistAggConv.  Every step keeps the overlap of
-    _gat_propagate with the two-pass marginal rows.  p2p transport only; the layer-0 evaluation cache does not apply
+    _propagate with the two-pass marginal rows.  p2p transport only; the layer-0 evaluation cache does not apply
     (z depends on the weights)."""
 
     @staticmethod
     def forward(ctx, z: Tensor, graph, k: int, alpha: float, is_train: bool) -> Tensor:
-        if comm.ctx.transport != "p2p":
-            raise NotImplementedError("APPNP runs on the p2p transport only (not the CPU gloo plumbing mode)")
-        eng = engine.ctx
+        _p2p_only("APPNP")
         z = z.contiguous()
-        g = graph.full if isinstance(graph, DecompGraph) else graph
-        quant = eng.bit_type == BitType.QUANT and is_train
+        g = _full(graph)
         h = z
         for step in range(k):
-            h = _teleport_step(f"forward{step}", quant, g, h, z, alpha, is_train)
+            h = _teleport_step(f"forward{step}", g, h, z, alpha, is_train)
         ctx.graph, ctx.k, ctx.alpha = graph, k, alpha
         return h
 
@@ -687,13 +649,12 @@ class DistAPPNPProp(Function):
     def backward(ctx: Any, *grad_outputs: Tuple[Tensor, ...]):
         grad = grad_outputs[0].contiguous()
         k, alpha = ctx.k, ctx.alpha
-        g = ctx.graph.full if isinstance(ctx.graph, DecompGraph) else ctx.graph
-        quant = engine.ctx.bit_type == BitType.QUANT
+        g = _full(ctx.graph)
         acc = torch.empty_like(grad)             # alpha * sum of the g_{k+1} seen so far
         nxt = grad                               # g_{k+1}
         for step in range(k - 1, -1, -1):
             mode = ACC_ON | (ACC_READ if step < k - 1 else 0) | (ACC_FOLD if step == 0 else 0)
-            nxt = _accum_step(f"backward{step}", quant, g, nxt, acc, alpha, mode)
+            nxt = _accum_step(f"backward{step}", g, nxt, acc, alpha, mode)
         return nxt, None, None, None, None
 
 
@@ -713,19 +674,14 @@ class DistGCNIIProp(Function):
 
     @staticmethod
     def forward(ctx, d: Tensor, h0: Tensor, graph, alpha: float, is_train: bool, layer: int) -> Tensor:
-        if comm.ctx.transport != "p2p":
-            raise NotImplementedError("GCNII runs on the p2p transport only (not the CPU gloo plumbing mode)")
-        g = graph.full if isinstance(graph, DecompGraph) else graph
-        quant = engine.ctx.bit_type == BitType.QUANT and is_train
-        s = _teleport_step(f"forward{layer}", quant, g, d.contiguous(), h0.contiguous(), alpha, is_train)
+        _p2p_only("GCNII")
+        s = _teleport_step(f"forward{layer}", _full(graph), d.contiguous(), h0.contiguous(), alpha, is_train)
         ctx.graph, ctx.alpha, ctx.layer = graph, alpha, layer
         return s
 
     @staticmethod
     def backward(ctx: Any, *grad_outputs: Tuple[Tensor, ...]):
         ds = grad_outputs[0].contiguous()
-        g = ctx.graph.full if isinstance(ctx.graph, DecompGraph) else ctx.graph
-        quant = engine.ctx.bit_type == BitType.QUANT
         dh0 = torch.empty_like(ds)
-        dd = _accum_step(f"backward{ctx.layer}", quant, g, ds, dh0, ctx.alpha, ACC_ON)
+        dd = _accum_step(f"backward{ctx.layer}", _full(ctx.graph), ds, dh0, ctx.alpha, ACC_ON)
         return dd, dh0, None, None, None, None

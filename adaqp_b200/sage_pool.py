@@ -19,6 +19,7 @@ import torch
 from torch import Tensor
 
 from . import _lib
+from .manager.graph import part_segments
 
 NO_ARG = -2 ** 31
 LAUNCHES = {"sage_pool_fwd_kernel": 0, "sage_pool_bwd_kernel": 0}
@@ -29,17 +30,6 @@ def _rows(t: Optional[Tensor], F: int, dtype=torch.float32) -> Optional[Tensor]:
         return None
     assert t.dtype == dtype and t.dim() == 2 and t.shape[1] == F and t.stride(1) == 1, (t.dtype, t.shape, t.stride())
     return t
-
-
-def _segments(graph, part: Optional[str]):
-    """(seg_start, seg_end, accumulate) of one launch, as in manager.graph.spmm."""
-    if part is None:
-        return None, None, 0
-    if part == "local":
-        return None, graph.halo_split.data_ptr(), 0
-    if part == "halo":
-        return graph.halo_split.data_ptr(), None, 1
-    raise ValueError(part)
 
 
 def forward(graph, x: Tensor, x_halo: Optional[Tensor], row_begin: int = 0, row_end: Optional[int] = None,
@@ -59,7 +49,7 @@ def forward(graph, x: Tensor, x_halo: Optional[Tensor], row_begin: int = 0, row_
     if arg is None:
         arg = torch.empty((n, F), dtype=torch.int32, device=x.device)
     assert out.stride(1) == 1 and arg.stride(1) == 1 and arg.dtype == torch.int32
-    seg_start, seg_end, acc = _segments(graph, part)
+    seg_start, seg_end, acc = part_segments(graph, part)
     rc = _lib.load().adaqp_sage_pool_fwd_f32(
         graph.indptr.data_ptr(), seg_start, seg_end, graph.indices.data_ptr(), graph.n_inner, x.data_ptr(),
         x.stride(0), x_halo.data_ptr() if x_halo is not None else None, x_halo.stride(0) if x_halo is not None else 0,
@@ -87,7 +77,7 @@ def backward(graph, want: Tensor, g: Tensor, g_halo: Optional[Tensor], arg: Tens
     if dp is None:
         dp = torch.empty((row_end - row_begin, F), dtype=torch.float32, device=g.device)
     assert dp.stride(1) == 1
-    seg_start, seg_end, acc = _segments(graph, part)
+    seg_start, seg_end, acc = part_segments(graph, part)
     rc = _lib.load().adaqp_sage_pool_bwd_f32(
         graph.indptr.data_ptr(), seg_start, seg_end, graph.indices.data_ptr(), want.data_ptr(), graph.n_inner,
         g.data_ptr(), g.stride(0), g_halo.data_ptr() if g_halo is not None else None,
