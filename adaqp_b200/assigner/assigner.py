@@ -13,7 +13,7 @@ from __future__ import annotations
 import logging
 import time
 from itertools import chain
-from typing import Dict, List, Tuple, Union
+from typing import Dict, Tuple, Union
 
 import numpy as np
 import torch
@@ -21,7 +21,7 @@ from torch import Tensor
 
 from ..communicator import BITS_SET
 from ..communicator import Communicator as comm
-from ..communicator.p2p import quantisable
+from ..communicator.p2p import layer_key_dims, quantisable
 from ..helper import BitType
 from ..manager import GraphEngine as engine
 from . import solver
@@ -32,11 +32,6 @@ logger = logging.getLogger("trainer")
 ASSIGNMENT_SCHEME = ("uniform", "random", "adaptive")
 
 
-def _layer_keys(num_layers: int) -> List[str]:
-    """forward0..L-1 then backward1..L-1 (layer 0 never sends gradients, :98-101)."""
-    return [f"forward{i}" for i in range(num_layers)] + [f"backward{i}" for i in range(1, num_layers)]
-
-
 class Assigner(object):
     ctx: "Assigner" = None
 
@@ -44,12 +39,11 @@ class Assigner(object):
                  uniform_assign_bits: int, scores: Dict[int, Tuple[Tensor, Tensor]], group_size: int,
                  coe_lambda: float, assign_cycle: int = None, warmup: int = 1, key_dims: Dict[str, int] = None):
         assert scheme in ASSIGNMENT_SCHEME, f"assignment scheme {scheme} is not supported"
-        # keys that travel quantised and their row widths: by default forward0..L-1 / backward1..L-1 with layer 0
-        # feat_dim wide; a model with its own exchange (GAT) passes every key's real width
+        # keys that travel quantised and their row widths: by default the reference's forward0..L-1 / backward1..L-1
+        # with layer 0 feat_dim wide; a model with its own exchange (GAT) passes every key's real width
         if key_dims is None:
-            self.key_dims = {k: (feat_dim if k.endswith("0") else hidden_dim) for k in _layer_keys(num_layers)}
-        else:
-            self.key_dims = {k: int(v) for k, v in key_dims.items() if quantisable(k)}
+            key_dims = layer_key_dims([feat_dim] + [hidden_dim] * (num_layers - 1))
+        self.key_dims = {k: int(v) for k, v in key_dims.items() if quantisable(k)}
         self.keys = list(self.key_dims)
         self.bits_set = torch.tensor(BITS_SET, dtype=torch.int32)
         self.bits_cost = torch.tensor([1 / (2 ** b - 1) ** 2 for b in BITS_SET], dtype=torch.float32)

@@ -57,6 +57,11 @@ def key_dim(key: str, buffer_shape: Sequence[int]) -> int:
     return int(buffer_shape[layer_index(key)])
 
 
+def layer_key_dims(buffer_shape: Sequence[int]) -> Dict[str, int]:
+    """The reference models' key table: layer_keys, each as wide as its layer's entry of buffer_shape."""
+    return {k: key_dim(k, buffer_shape) for k in layer_keys(len(buffer_shape))}
+
+
 def attn_keys(layer: int) -> Tuple[str, str]:
     """fp32 keys of GAT's per-row attention scalars: el rows with the forward exchange, [er | lse | s] rows with the
     backward exchange.  Training and evaluation never have the same key in flight, so both use them."""
@@ -385,7 +390,7 @@ class PeerExchange:
     (conversion.py:92-106, processing.py:53-60).  `gather(obj) -> list` is the control
     plane all_gather (comm.all_gather_any in multi-process runs; tests wire ranks
     in-process through `connect`).  `key_dims` (ordered key -> row width, e.g. gat_key_dims) replaces the
-    default keys of layer_keys with widths from buffer_shape."""
+    default table, layer_key_dims(buffer_shape)."""
 
     def __init__(self, rank: int, world_size: int, device: torch.device, buffer_shape: Sequence[int],
                  send_idx: Dict[int, Tuple[int, int]], recv_idx: Dict[int, torch.Tensor],
@@ -395,11 +400,9 @@ class PeerExchange:
         self.buffer_shape = [int(x) for x in buffer_shape]
         self.num_layers = len(self.buffer_shape)
         if key_dims is None:
-            self.keys = layer_keys(self.num_layers)
-            self.dims = {k: key_dim(k, self.buffer_shape) for k in self.keys}
-        else:
-            self.keys = list(key_dims)
-            self.dims = {k: int(v) for k, v in key_dims.items()}
+            key_dims = layer_key_dims(self.buffer_shape)
+        self.keys = list(key_dims)
+        self.dims = {k: int(v) for k, v in key_dims.items()}
         self.send_idx = {int(p): (int(lo), int(hi)) for p, (lo, hi) in send_idx.items()}
         self.recv_idx = {int(p): torch.as_tensor(v).cpu().numpy().astype(np.int64) for p, v in recv_idx.items()}
         self.total_send_idx = torch.as_tensor(total_send_idx).cpu().numpy().astype(np.int64)

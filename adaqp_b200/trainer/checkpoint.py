@@ -21,10 +21,11 @@ import numpy as np
 import torch
 
 from ..assigner import Assigner as assigner
-from ..assigner.assigner import _layer_keys
 from ..communicator import Communicator as comm
+from ..communicator.p2p import layer_key_dims, quantisable
 from ..helper import BitType
 from ..manager import GraphEngine as engine
+from ..model.registry import MODELS
 
 FORMAT_VERSION = 1
 # what a resumed run must share with the run that wrote the checkpoint; the first five also fix the weights' shapes
@@ -43,23 +44,14 @@ def run_fields(config: dict, key_dims: Optional[Dict[str, int]]) -> dict:
     (None: the reference's keys, as the Assigner builds them)."""
     data, model, rt = config["data"], config["model"], config["runtime"]
     L, H = int(model["num_layers"]), int(model["hidden_dim"])
+    layer_dims = [int(data["num_feats"])] + [H] * (L - 1) + [int(data["num_classes"])]
     if key_dims is None:
-        key_dims = {k: (data["num_feats"] if k.endswith("0") else H) for k in _layer_keys(L)}
+        key_dims = {k: v for k, v in layer_key_dims(layer_dims[:-1]).items() if quantisable(k)}
     return {"dataset": rt["dataset"], "model_name": rt["model_name"], "aggregator_type": model["aggregator_type"],
-            "gat_heads": int(model["gat_heads"]), "layer_dims": [int(data["num_feats"])] + [H] * (L - 1) + [int(data["num_classes"])],
+            "gat_heads": int(model["gat_heads"]), "layer_dims": layer_dims,
             "num_parts": int(rt["num_parts"]), "mode": rt["mode"], "assign_scheme": rt["assign_scheme"],
             "key_dims": {k: int(v) for k, v in key_dims.items()},
-            "propagation": _propagation(rt["model_name"], model)}
-
-
-def _propagation(model_name: str, model: dict) -> Optional[dict]:
-    """The propagation parameters of the models that have them (None for the others)."""
-    if model_name == "appnp":
-        return {"k": int(model["appnp_k"]), "alpha": float(model["appnp_alpha"])}
-    if model_name == "gcnii":
-        return {"layers": int(model["gcnii_layers"]), "alpha": float(model["gcnii_alpha"]),
-                "theta": float(model["gcnii_theta"])}
-    return None
+            "propagation": MODELS[rt["model_name"]].propagation(config)}
 
 
 def partition_digest(layout) -> dict:

@@ -17,16 +17,12 @@ from torch import Tensor
 
 from ..assigner import Assigner as assigner
 from ..communicator import Communicator as comm
-from ..helper import BitType, DistGNNType
-from .. import gatv2, sage_pool
-from ..manager import DecompGraph
+from ..helper import BitType
 from ..manager import GraphEngine as engine
-from ..communicator.p2p import appnp_key_dims, gat_key_dims, gatv2_key_dims, sage_pool_key_dims
-from ..model import DistAPPNP, DistGAT, DistGATv2, DistGCN, DistGCNII, DistSAGE
-from ..model.distAPPNP import APPNP_ALPHA, APPNP_K, appnp_params
-from ..model.distGCNII import GCNII_ALPHA, GCNII_LAYERS, GCNII_THETA, gcnii_params
+from ..model.distAPPNP import APPNP_ALPHA, APPNP_K
+from ..model.distGCNII import GCNII_ALPHA, GCNII_LAYERS, GCNII_THETA
+from ..model.registry import MODELS, buffer_shape
 from ..manager.graphEngine import load_rank_layout
-from ..model.distGAT import gat_layer_shapes
 from . import checkpoint as ckpt
 from .runtime_util import (_check_exchange_status, aggregate_accuracy, aggregate_F1, get_metrics, setup_logger,
                            sync_model, sync_seed, train_for_one_epoch, val_test)
@@ -35,10 +31,6 @@ RUNING_MODE = ["Vanilla", "AdaQP", "AdaQP-q", "AdaQP-p"]
 # mode -> (message precision, overlap central aggregation with the exchange)
 QUNAT_PARA_MAP: Dict[str, Tuple[str, bool]] = {"Vanilla": ("full", False), "AdaQP": ("quant", True),
                                                "AdaQP-q": ("quant", False), "AdaQP-p": ("full", True)}
-# 'gat', 'appnp', 'gcnii' and 'gatv2' are extensions beyond the reference's two models
-MODEL_MAP: Dict[str, DistGNNType] = {"gcn": DistGNNType.DistGCN, "sage": DistGNNType.DistSAGE, "gat": DistGNNType.DistGAT,
-                                     "appnp": DistGNNType.DistAPPNP, "gcnii": DistGNNType.DistGCNII,
-                                     "gatv2": DistGNNType.DistGATv2}
 GAT_HEADS = 4          # default of the yaml `model: gat_heads`
 
 
@@ -99,37 +91,26 @@ class Trainer(object):
         data, rt, model = self.config["data"], self.config["runtime"], self.config["model"]
         if rt["mode"] not in RUNING_MODE:
             raise ValueError(f"Invalid running mode: {rt['mode']}")
-        if rt["model_name"] not in MODEL_MAP:
+        self.spec = MODELS.get(rt["model_name"])
+        if self.spec is None:
             raise ValueError(f"Invalid model type: {rt['model_name']}")
-        if MODEL_MAP[rt["model_name"]] in (DistGNNType.DistGAT, DistGNNType.DistGATv2):
-            gat_layer_shapes(model["hidden_dim"], data["num_classes"], model["num_layers"], model["gat_heads"])
-            if comm.ctx.transport != "p2p":
-                raise NotImplementedError(f"model '{rt['model_name']}' runs on the p2p transport only; the CPU gloo "
-                                          "plumbing mode (ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports gcn and sage")
-        if self._is_appnp():
-            appnp_params(model["appnp_k"], model["appnp_alpha"])
-            if comm.ctx.transport != "p2p":
-                raise NotImplementedError("model 'appnp' runs on the p2p transport only; the CPU gloo plumbing mode "
-                                          "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports gcn and sage")
-        if self._is_gcnii():
-            gcnii_params(model["gcnii_layers"], model["gcnii_alpha"], model["gcnii_theta"])
-            if comm.ctx.transport != "p2p":
-                raise NotImplementedError("model 'gcnii' runs on the p2p transport only; the CPU gloo plumbing mode "
-                                          "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports gcn and sage")
-        if self._is_pool() and comm.ctx.transport != "p2p":
-            raise NotImplementedError("aggregator_type 'pool' runs on the p2p transport only; the CPU gloo plumbing mode "
-                                      "(ADAQP_DEVICE=cpu / ADAQP_TRANSPORT=gloo) supports the mean and gcn aggregators")
+        self.spec.check(self.config)
+        refusal = self.spec.p2p_only(self.config)
+        if refusal is not None and comm.ctx.transport != "p2p":
+            raise NotImplementedError(refusal)
+        # the model's own exchange keys and widths (None: the reference's, built from buffer_shape)
+        self.key_dims = self.spec.key_dims(self.config)
         precision, use_parallel = QUNAT_PARA_MAP[rt["mode"]]
         layout = None
         if rt["resume"]:
             # a checkpoint that does not belong to this run is refused before any device work or exchange
-            layout = load_rank_layout(data["partition_path"], rt["dataset"], MODEL_MAP[rt["model_name"]])
+            layout = load_rank_layout(data["partition_path"], rt["dataset"], self.spec.kind)
             self._partition_digest = ckpt.partition_digest(layout)
             self.resume_path = ckpt.resolve(rt["resume"], rt["checkpoint_dir"])
             self.resume_epoch = ckpt.check_resume(self.resume_path, self.run_fields(), self._partition_digest,
                                                   rt["num_epoches"])
         self.engine = engine(rt["num_epoches"], data["partition_path"], rt["dataset"], precision,
-                             MODEL_MAP[rt["model_name"]], use_parallel, layout=layout)
+                             self.spec.kind, use_parallel, layout=layout)
         engine.ctx.agg_type = model["aggregator_type"]
         engine.ctx.top_layer = model["num_layers"] - 1
         if engine.ctx.use_parallel:
@@ -138,121 +119,25 @@ class Trainer(object):
         self.logger.info(repr(self.engine))
 
     def _set_buffer(self):
-        data, model = self.config["data"], self.config["model"]
-        shape = [data["num_feats"]] + [model["hidden_dim"]] * (model["num_layers"] - 1)
-        extra = {}
-        if self._is_gat():
-            # GAT exchanges the projected rows z of every layer (plus backward0 and the attention scalars)
-            shape, heads = self._gat_shapes()
-            extra["key_dims"] = gat_key_dims(shape, heads)
-        elif self._is_gatv2():
-            # GATv2 exchanges the source projection zs of every layer and pushes its halo gradients back
-            shape, _ = self._gat_shapes()
-            extra["key_dims"] = self._key_dims()
-        elif self._is_pool():
-            # max-pool exchanges the pooled rows p of every layer (plus backward0 and the arg rows)
-            extra["key_dims"] = self._key_dims()
-        elif self._is_appnp():
-            # APPNP exchanges num_classes-wide rows at each of its K steps: one fp32 test{k} buffer per step
-            shape = [data["num_classes"]] * int(model["appnp_k"])
-            extra["key_dims"] = self._key_dims()
-        elif self._is_gcnii():
-            # GCNII exchanges hidden-width rows at each of its L layers: one fp32 test{l} buffer per layer
-            shape = [model["hidden_dim"]] * int(model["gcnii_layers"])
-            extra["key_dims"] = self._key_dims()
-        comm.ctx.init_buffer(shape, engine.ctx.send_idx, engine.ctx.recv_idx, engine.ctx.bit_type,
-                             total_send_idx=engine.ctx.total_send_idx, num_remote=engine.ctx.num_remove, **extra)
-        if self._is_pool():
-            self._set_pool_want()
-        if self._is_gatv2():
-            self._set_gatv2_tables()
-
-    def _set_pool_want(self):
-        """The backward match table of the max-pool aggregation, aligned with the CSR the kernels read; the peers'
-        recv_idx come from the exchange's set-up all-gather."""
-        eng, ex = engine.ctx, comm.ctx.comm_buffer.p2p
-        g = eng.graph.full if isinstance(eng.graph, DecompGraph) else eng.graph
-        want = sage_pool.pool_want(g.indptr.cpu().numpy(), g.indices.cpu().numpy(), g.n_inner, ex.recv_idx,
-                                   ex.send_idx, ex.total_send_idx, ex.peer_recv_idx)
-        eng.pool_want = torch.from_numpy(want).to(g.device)
-
-    def _set_gatv2_tables(self):
-        """GATv2's backward tables, aligned with the CSR the kernels read: the halo-transposed CSR (the inner
-        destinations of every halo row) and the fold table (the push-region rows of every inner row)."""
-        eng, ex = engine.ctx, comm.ctx.comm_buffer.p2p
-        g = eng.graph.full if isinstance(eng.graph, DecompGraph) else eng.graph
-        hp, hd = gatv2.halo_table(g.indptr.cpu().numpy(), g.indices.cpu().numpy(), g.n_inner, ex.num_remote)
-        fp, fpos = gatv2.fold_table(g.n_inner, ex.send_peers, ex.send_idx, ex.total_send_idx)
-        eng.gatv2_halo = tuple(torch.from_numpy(a).to(g.device) for a in (hp, hd))
-        eng.gatv2_fold = tuple(torch.from_numpy(a).to(g.device) for a in (fp, fpos))
-
-    def _is_gat(self) -> bool:
-        return MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistGAT
-
-    def _is_gatv2(self) -> bool:
-        return MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistGATv2
-
-    def _is_appnp(self) -> bool:
-        return MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistAPPNP
-
-    def _is_gcnii(self) -> bool:
-        return MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistGCNII
-
-    def _is_pool(self) -> bool:
-        return (MODEL_MAP[self.config["runtime"]["model_name"]] == DistGNNType.DistSAGE
-                and self.config["model"]["aggregator_type"] == "pool")
-
-    def _key_dims(self):
-        """Per-key exchange widths of the models with their own exchange protocol (None: the reference's keys)."""
-        if self._is_gat():
-            return gat_key_dims(*self._gat_shapes())
-        if self._is_gatv2():
-            return gatv2_key_dims(self._gat_shapes()[0])
-        if self._is_pool():
-            data, model = self.config["data"], self.config["model"]
-            return sage_pool_key_dims([data["num_feats"]] + [model["hidden_dim"]] * (model["num_layers"] - 1))
-        if self._is_appnp():
-            return appnp_key_dims(self.config["data"]["num_classes"], int(self.config["model"]["appnp_k"]))
-        if self._is_gcnii():
-            # the same key table as APPNP's: test / forward / backward 0 .. L-1, all hidden_dim wide
-            return appnp_key_dims(self.config["model"]["hidden_dim"], int(self.config["model"]["gcnii_layers"]))
-        return None
-
-    def _gat_shapes(self):
-        data, model = self.config["data"], self.config["model"]
-        return gat_layer_shapes(model["hidden_dim"], data["num_classes"], model["num_layers"], model["gat_heads"])
+        comm.ctx.init_buffer(buffer_shape(self.config, self.key_dims), engine.ctx.send_idx, engine.ctx.recv_idx,
+                             engine.ctx.bit_type, total_send_idx=engine.ctx.total_send_idx,
+                             num_remote=engine.ctx.num_remove, key_dims=self.key_dims)
+        self.spec.setup(engine.ctx, comm.ctx.comm_buffer.p2p)
 
     def run_fields(self) -> dict:
         """What a checkpoint's manifest records about the run (trainer/checkpoint.py)."""
-        return ckpt.run_fields(self.config, self._key_dims())
+        return ckpt.run_fields(self.config, self.key_dims)
 
     def _set_assigner(self):
         data, model, rt, asg = (self.config[k] for k in ("data", "model", "runtime", "assignment"))
         self.assigner = assigner(data["num_feats"], model["hidden_dim"], model["num_layers"],
                                  asg["profile_data_length"], rt["assign_scheme"], asg["assign_bits"],
                                  engine.ctx.scores, asg["group_size"], asg["coe_lambda"], asg["assign_cycle"],
-                                 key_dims=self._key_dims())
+                                 key_dims=self.key_dims)
         self.logger.info(self.assigner)
 
     def _set_model(self):
-        data, model, rt = self.config["data"], self.config["model"], self.config["runtime"]
-        kind = MODEL_MAP[rt["model_name"]]
-        common = (data["num_feats"], model["hidden_dim"], data["num_classes"], model["num_layers"],
-                  model["dropout_rate"], model["use_norm"])
-        if kind == DistGNNType.DistGCN:
-            self.model = DistGCN(*common).to(comm.ctx.device)
-        elif kind == DistGNNType.DistGAT:
-            self.model = DistGAT(*common, heads=model["gat_heads"]).to(comm.ctx.device)
-        elif kind == DistGNNType.DistGATv2:
-            self.model = DistGATv2(*common, heads=model["gat_heads"]).to(comm.ctx.device)
-        elif kind == DistGNNType.DistAPPNP:
-            self.model = DistAPPNP(*common, k=model["appnp_k"], alpha=model["appnp_alpha"]).to(comm.ctx.device)
-        elif kind == DistGNNType.DistGCNII:
-            self.model = DistGCNII(data["num_feats"], model["hidden_dim"], data["num_classes"], model["dropout_rate"],
-                                   layers=model["gcnii_layers"], alpha=model["gcnii_alpha"],
-                                   theta=model["gcnii_theta"]).to(comm.ctx.device)
-        else:
-            self.model = DistSAGE(*common, model["aggregator_type"]).to(comm.ctx.device)
+        self.model = self.spec.build(self.config).to(comm.ctx.device)
 
     # ---- runtime ----------------------------------------------------------------------------------
     def train(self):

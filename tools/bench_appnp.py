@@ -120,7 +120,7 @@ def _train_worker(rank, world, port, tmp, mode, scale, epochs, out):
                            model_name="appnp", mode=mode, assign_scheme="uniform", logger_level="WARNING",
                            num_epoches=epochs, exp_path=f"{tmp}/exp"))
     C = tr.config["data"]["num_classes"]
-    keys = [k for k in tr._key_dims() if k.startswith(("forward", "backward"))]
+    keys = [k for k in tr.key_dims if k.startswith(("forward", "backward"))]
     wire = _wire_bytes(C, keys)
     rec = tr.train()
     out.put((rank, (float(rec[2]), float(np.mean(tr.exposed_comm_ms)), wire)))

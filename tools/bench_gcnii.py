@@ -127,7 +127,7 @@ def _train_worker(rank, world, port, tmp, mode, scale, epochs, out):
                                model_name="gcnii", mode=mode, assign_scheme="uniform", logger_level="WARNING",
                                num_epoches=epochs, exp_path=f"{tmp}/exp"))
         H = tr.config["model"]["hidden_dim"]
-        keys = [k for k in tr._key_dims() if k.startswith(("forward", "backward"))]
+        keys = [k for k in tr.key_dims if k.startswith(("forward", "backward"))]
         wire = _wire_bytes(H, keys)
         torch.cuda.synchronize()
         torch.cuda.reset_peak_memory_stats()
