@@ -20,7 +20,7 @@ i32 = C.c_int32
 u64 = C.c_uint64
 u32 = C.c_uint32
 
-ADAQP_ABI_VERSION = 8
+ADAQP_ABI_VERSION = 9
 MAX_PARTS = 64           # ADAQP_MAX_PARTS
 LP_HUB_DEGREE = 256      # ADAQP_LP_HUB_DEGREE
 IPC_HANDLE_BYTES = 64
@@ -89,6 +89,13 @@ SYMBOLS = {
     "adaqp_appnp_prop_f32": (C.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, i64, i64, c_void_p, i64,
                                        c_void_p, c_void_p, C.c_float, C.c_float, c_void_p, i64, c_void_p, i64, i32,
                                        C.c_int, i64, i64, i32, c_void_p, i64, c_void_p]),
+    "adaqp_cs_prop_f32": (C.c_int, [c_void_p, c_void_p, c_void_p, i64, i64, c_void_p, i64, c_void_p, c_void_p,
+                                    C.c_float, C.c_float, c_void_p, i64, c_void_p, c_void_p, i64, i32, C.c_float,
+                                    C.c_float, i64, i64, i32, c_void_p, i64, c_void_p]),
+    "adaqp_cs_init_f32": (C.c_int, [c_void_p, i64, c_void_p, i64, i32, c_void_p, i64, c_void_p, i64, c_void_p, i32,
+                                    c_void_p]),
+    "adaqp_cs_combine_f32": (C.c_int, [c_void_p, i64, c_void_p, i64, c_void_p, i64, i32, i32, C.c_double, c_void_p,
+                                       i64, c_void_p]),
     "adaqp_gemm_tf32x3_supported": (C.c_int, [i64, i32, i32, i64, i64, i64]),
     "adaqp_gemm_tf32x3_f32": (C.c_int, [c_void_p, i64, c_void_p, c_void_p, i64, c_void_p, i64, i32, i32, c_void_p, i64, c_void_p]),
     "adaqp_wgrad_tf32x3_supported": (C.c_int, [i64, i32, i32, i64, i64]),

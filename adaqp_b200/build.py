@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "_build")
 LIB = os.path.join(HERE, "libadaqp_b200.so")
 SOURCES = ["runtime.cu", "quant.cu", "exchange.cu", "spmm.cu", "gemm.cu", "norm.cu", "partition.cu", "gat.cu", "sage_pool.cu",
-           "gatv2.cu"]
+           "gatv2.cu", "cs.cu"]
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "attn.cuh"),
            os.path.join(os.path.dirname(HERE), "include", "adaqp_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

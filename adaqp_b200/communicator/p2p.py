@@ -132,6 +132,15 @@ def gatv2_key_dims(widths: Sequence[int]) -> Dict[str, int]:
     return dims
 
 
+# fp32 key of Correct & Smooth's propagation steps (model/ops.py correct_and_smooth): every step of a pass reuses it
+CS_KEY = "cs0"
+
+
+def with_cs_key(key_dims: Dict[str, int], num_classes: int) -> Dict[str, int]:
+    """A key table with CS_KEY appended, num_classes wide."""
+    return {**key_dims, CS_KEY: int(num_classes)}
+
+
 def quantisable(key: str) -> bool:
     """Keys that may travel quantised (training exchanges of layer rows); test, attention and arg keys are fp32."""
     return key.startswith(("forward", "backward"))

@@ -310,6 +310,89 @@ appnp_prop_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict_
 }
 
 // ---------------------------------------------------------------------------------------
+// Correct & Smooth propagation step (DESIGN §16): appnp_prop_kernel's teleport step, whole rows only (one pass per
+// row, no segments), followed by a non-linear post-step that two partial sums of a row could not take:
+//   r[v] = (scale * post[v]) * sum_{u in N(v)} pre[u] x[u]  (+ alpha * tele[v])
+//   POST = kCsClamp: out[v] = fminf(fmaxf(r[v], lo), hi)
+//   POST = kCsFix  : out[v] = fix[v] where y[v] >= 0 (the row's gather is skipped), else r[v]; tele is not read
+//                    (the fixed rows are the only rows where the correct step's E0 is nonzero)
+// tele, fix, y and out are indexed by v - row_begin.  The gather and the fmul / fmaf of the epilogue are those of
+// appnp_prop_kernel, so with lo = -inf and hi = +inf the clamp step is bitwise its teleport step.  The row's own
+// operands (tele; y and fix) are loaded before the gather.  Rows of at most 2 floats per lane are held to 40 registers
+// (6 CTAs per SM) and <4, 1> to 48 (5 CTAs), as appnp_prop_kernel; <1, 4> and <2, 2> to 64 (4 CTAs): at 48 they spill.
+constexpr int kCsClamp = 0;
+constexpr int kCsFix = 1;
+
+template <int VEC, int CHUNKS, int POST>
+__global__ void __launch_bounds__(kThreads, VEC * CHUNKS <= 2 ? 6 : (VEC == 4 && CHUNKS == 1 ? 5 : (VEC * CHUNKS <= 4 ? 4 : 1)))
+cs_prop_kernel(const int64_t *__restrict__ indptr, const int32_t *__restrict__ indices,
+               const float *__restrict__ x0, int64_t ld0, int64_t n_split,
+               const float *__restrict__ x1, int64_t ld1,
+               const float *__restrict__ pre, const float *__restrict__ post, float scale, float alpha,
+               const float *__restrict__ tele, int64_t ldt, const int32_t *__restrict__ y,
+               const float *__restrict__ fix, int64_t ldf, float lo, float hi,
+               int64_t row_begin, int64_t row_end, int F,
+               float *__restrict__ out, int64_t ldo, unsigned long long *__restrict__ next_row) {
+    const int lane = threadIdx.x & 31;
+    bool colok[CHUNKS];
+#pragma unroll
+    for (int c = 0; c < CHUNKS; ++c) colok[c] = ((c * 32 + lane) * VEC) < F;
+    const int64_t n_rows = row_end - row_begin;
+    const bool add_tele = POST == kCsClamp && tele != nullptr;
+    while (true) {
+        unsigned long long grab = 0;
+        if (lane == 0) grab = atomicAdd(next_row, 1ull);
+        grab = __shfl_sync(ADAQP_FULL_MASK, grab, 0);
+        if ((int64_t)grab >= n_rows) break;
+        const int64_t row = row_begin + (int64_t)grab;
+        const int64_t o = row - row_begin;
+        float *orow = out + o * ldo;
+        if (POST == kCsFix && __ldg(y + o) >= 0) {
+            // a fixed row: its E0 row, no gather
+#pragma unroll
+            for (int c = 0; c < CHUNKS; ++c) {
+                if (!colok[c]) continue;
+                const int col = (c * 32 + lane) * VEC;
+                float v[VEC];
+                Vec<VEC>::load(fix + o * ldf + col, v);
+                Vec<VEC>::store(orow + col, v);
+            }
+            continue;
+        }
+        float addend[CHUNKS][VEC];
+#pragma unroll
+        for (int c = 0; c < CHUNKS; ++c) {
+#pragma unroll
+            for (int e = 0; e < VEC; ++e) addend[c][e] = 0.f;
+            if (add_tele && colok[c]) Vec<VEC>::load(tele + o * ldt + (c * 32 + lane) * VEC, addend[c]);
+        }
+        float acc[CHUNKS][VEC];
+#pragma unroll
+        for (int c = 0; c < CHUNKS; ++c)
+#pragma unroll
+            for (int e = 0; e < VEC; ++e) acc[c][e] = 0.f;
+        const int64_t b = __ldg(indptr + row);
+        const int64_t e_ = __ldg(indptr + row + 1);
+        const int hints = 0;
+        ADAQP_GATHER_SEGMENT(kUnroll, false, nullptr)
+        const float s = post ? __fmul_rn(scale, __ldg(post + row)) : scale;
+#pragma unroll
+        for (int c = 0; c < CHUNKS; ++c) {
+            if (!colok[c]) continue;
+            float r[VEC];
+#pragma unroll
+            for (int e = 0; e < VEC; ++e) {
+                r[e] = __fmul_rn(acc[c][e], s);
+                if (add_tele) r[e] = __fmaf_rn(alpha, addend[c][e], r[e]);
+                if (POST == kCsClamp) r[e] = fminf(fmaxf(r[e], lo), hi);
+            }
+            Vec<VEC>::store(orow + (c * 32 + lane) * VEC, r);
+        }
+    }
+    frontier_release(next_row);
+}
+
+// ---------------------------------------------------------------------------------------
 // Column-sliced gather (the default path for 16-byte rows of 256, 384, ... columns, DESIGN §3).
 //
 // The F columns are aggregated as ceil(F / slice_cols) slices of at most slice_cols <= 128 columns in
@@ -1253,6 +1336,74 @@ int adaqp_appnp_prop_f32(const int64_t *indptr, const int64_t *seg_start, const 
     }
 #undef APPNP_PICK
     return adaqp_check_launch("appnp_prop_kernel");
+}
+
+int adaqp_cs_prop_f32(const int64_t *indptr, const int32_t *indices, const float *x0, int64_t ld0, int64_t n_split,
+                      const float *x1, int64_t ld1, const float *pre, const float *post, float scale, float alpha,
+                      const float *tele, int64_t ldt, const int32_t *y, const float *fix, int64_t ldf,
+                      int32_t post_mode, float lo, float hi, int64_t row_begin, int64_t row_end, int32_t F,
+                      float *out, int64_t ldo, void *stream) {
+    ADAQP_REQUIRE(F > 0 && F <= 1024, ADAQP_EINVAL, "adaqp_cs_prop_f32: C=%d outside [1, 1024]", F);
+    ADAQP_REQUIRE(row_end >= row_begin && row_begin >= 0 && row_end <= n_split, ADAQP_EINVAL,
+                  "adaqp_cs_prop_f32: bad row range [%lld, %lld) for n_split=%lld", (long long)row_begin,
+                  (long long)row_end, (long long)n_split);
+    ADAQP_REQUIRE(post_mode == kCsClamp || post_mode == kCsFix, ADAQP_EINVAL, "adaqp_cs_prop_f32: bad post_mode %d",
+                  post_mode);
+    ADAQP_REQUIRE(post_mode != kCsClamp || lo <= hi, ADAQP_EINVAL, "adaqp_cs_prop_f32: clamp bounds lo=%g > hi=%g",
+                  (double)lo, (double)hi);
+    if (row_end == row_begin) return 0;
+    ADAQP_REQUIRE(indptr && indices && x0 && out, ADAQP_EINVAL, "adaqp_cs_prop_f32: null pointer");
+    ADAQP_REQUIRE(post_mode != kCsFix || (y && fix), ADAQP_EINVAL, "adaqp_cs_prop_f32: null pointer (y / fix)");
+    if (post_mode == kCsFix) tele = nullptr;
+    int vec = 4;
+    auto fits = [&](int v) {
+        if (F % v || ld0 % v || ldo % v) return false;
+        if (!aligned(x0, v) || !aligned(out, v)) return false;
+        if (x1 && (!aligned(x1, v) || (ld1 % v))) return false;
+        if (tele && (!aligned(tele, v) || (ldt % v))) return false;
+        if (fix && (!aligned(fix, v) || (ldf % v))) return false;
+        return true;
+    };
+    while (vec > 1 && !fits(vec)) vec >>= 1;
+    const int nchunks = (F + 32 * vec - 1) / (32 * vec);
+    int dev = 0;
+    ADAQP_CUDA(cudaGetDevice(&dev));
+    cudaStream_t s = (cudaStream_t)stream;
+    unsigned long long *counter = frontier_counter(dev, s);
+    ADAQP_REQUIRE(counter != nullptr, ADAQP_EINVAL, "adaqp_cs_prop_f32: row counter allocation failed");
+    const int64_t grid = adaqp_frontier_grid(row_end - row_begin, kWarps);
+    auto launch = [&](auto kernel) {
+        kernel<<<(unsigned)grid, kThreads, 0, s>>>(indptr, indices, x0, ld0, n_split, x1, ld1, pre, post, scale, alpha,
+                                                   tele, ldt, y, fix, ldf, lo, hi, row_begin, row_end, F, out, ldo,
+                                                   counter);
+    };
+#define CS_PICK(V, C)                                                                                       \
+    do {                                                                                                    \
+        if (post_mode == kCsClamp) launch(cs_prop_kernel<V, C, kCsClamp>);                                  \
+        else launch(cs_prop_kernel<V, C, kCsFix>);                                                          \
+    } while (0)
+    // the ladder of appnp_prop_kernel: the narrowest instantiation that holds the row
+    if (vec == 4) {
+        if (nchunks <= 1) CS_PICK(4, 1);
+        else if (nchunks <= 2) CS_PICK(4, 2);
+        else if (nchunks <= 4) CS_PICK(4, 4);
+        else CS_PICK(4, 8);
+    } else if (vec == 2) {
+        if (nchunks <= 1) CS_PICK(2, 1);
+        else if (nchunks <= 2) CS_PICK(2, 2);
+        else if (nchunks <= 4) CS_PICK(2, 4);
+        else if (nchunks <= 8) CS_PICK(2, 8);
+        else CS_PICK(2, 16);
+    } else {
+        if (nchunks <= 1) CS_PICK(1, 1);
+        else if (nchunks <= 2) CS_PICK(1, 2);
+        else if (nchunks <= 4) CS_PICK(1, 4);
+        else if (nchunks <= 8) CS_PICK(1, 8);
+        else if (nchunks <= 16) CS_PICK(1, 16);
+        else CS_PICK(1, 32);
+    }
+#undef CS_PICK
+    return adaqp_check_launch("cs_prop_kernel");
 }
 
 }  // extern "C"

@@ -12,15 +12,16 @@ aggregate on the default stream; ordering is by CUDA events only.
 from __future__ import annotations
 
 import contextlib
+import math
 from typing import Any, Optional, Tuple
 
 import torch
 from torch import Tensor
 from torch.autograd import Function
 
-from .. import gat, gatv2, sage_pool
+from .. import cs, gat, gatv2, sage_pool
 from ..communicator import Communicator as comm
-from ..communicator.p2p import attn_keys, pool_arg_key, push_key
+from ..communicator.p2p import CS_KEY, attn_keys, pool_arg_key, push_key
 from ..helper import BitType, ProprogationMode
 from ..manager import DecompGraph
 from ..manager import GraphEngine as engine
@@ -605,6 +606,59 @@ def _teleport_step(name: str, g: LocalGraph, h: Tensor, z: Tensor, alpha: float,
 
     _propagate(name, _comm_name(name, is_train), _exchange(h, name, is_train), aggregate, split=True, sent=(h,))
     return out
+
+
+def _cs_step(step: int, g: LocalGraph, x: Tensor, alpha: float, tele: Tensor = None, y: Tensor = None,
+             fix: Tensor = None, lo: float = -math.inf, hi: float = math.inf) -> Tensor:
+    """One Correct & Smooth step over the fp32 exchange of x on CS_KEY (A with the GCN forward norms):
+    out = clamp(alpha A x + (1 - alpha) tele, lo, hi), or with `fix` out = alpha A x with every row of y >= 0 reset to
+    its row of fix.  The central rows run while the exchange is in flight; the marginal rows run in one pass once the
+    halo has landed: a clamp or a fixed row cannot be applied to two partial sums.  Every step of a pass reuses the
+    key; its sequence numbers pace them.  `step` names the timer regions."""
+    ex = comm.ctx.comm_buffer.p2p
+    pre, post = g.norm["out_-0.5"], g.norm["in_-0.5"]
+    out = torch.empty_like(x)
+
+    def exchange(stream):
+        ex.post_send_fp(CS_KEY, x, stream=stream)
+        return ex.complete_recv_fp(CS_KEY, stream=stream), None, lambda: ex.release_fp(CS_KEY)
+
+    def aggregate(lo_, hi_, halo, _, part=None):
+        cs.prop(g, x, halo, pre, post, alpha, 1.0 - alpha, lo_, hi_, out[lo_:hi_],
+                tele=tele[lo_:hi_] if tele is not None else None, y=y[lo_:hi_] if y is not None else None,
+                fix=fix[lo_:hi_] if fix is not None else None, lo=lo, hi=hi)
+
+    name = f"cs{step}"
+    _propagate(name, f"{name}_communication", exchange, aggregate, sent=(x,))
+    return out
+
+
+def correct_and_smooth(graph, logits: Tensor, y: Tensor, params: "cs.CSParams", n_train: int) -> Tensor:
+    """Correct & Smooth (DESIGN §16) of this rank's [n_inner, C] base logits; every rank calls it together.  `y`:
+    int32 per inner row, the label of the rank's train rows and -1 elsewhere; `n_train`: the train rows of all ranks.
+    Returns the smoothed probabilities G_K.  fp32 exchange in every mode; p2p transport only."""
+    _p2p_only("Correct & Smooth")
+    g = _full(graph)
+    z = logits.detach().float().contiguous()
+    yhat, e0, l1 = cs.init(z, y)
+    total = torch.tensor([l1], dtype=torch.float64)
+    comm.all_reduce_sum(total)
+    sigma = float(total[0]) / max(int(n_train), 1)
+    a1, a2 = params.correct_alpha, params.smooth_alpha
+    e, step = e0, 0
+    for _ in range(params.correct_layers):
+        if params.scale is None:
+            e = _cs_step(step, g, e, a1, tele=e0, lo=-1.0, hi=1.0)
+        else:
+            e = _cs_step(step, g, e, a1, y=y, fix=e0)
+        step += 1
+    g0 = cs.combine(yhat, e, y, sigma=sigma) if params.scale is None else cs.combine(yhat, e, y, scale=params.scale)
+    h = g0
+    for _ in range(params.smooth_layers):
+        h = _cs_step(step, g, h, a2, tele=g0, lo=0.0, hi=1.0)
+        step += 1
+    engine.ctx.timer.clear(is_train=False)
+    return h
 
 
 def _accum_step(name: str, g: LocalGraph, grad: Tensor, acc: Tensor, alpha: float, mode: int) -> Tensor:

@@ -8,7 +8,7 @@ import csv
 import json
 import os
 from argparse import Namespace
-from typing import Dict, Tuple
+from typing import Dict, Optional, Tuple
 
 import numpy as np
 import torch
@@ -17,10 +17,13 @@ from torch import Tensor
 
 from ..assigner import Assigner as assigner
 from ..communicator import Communicator as comm
+from ..communicator.p2p import layer_key_dims, with_cs_key
+from ..cs import CSParams, cs_params
 from ..helper import BitType
 from ..manager import GraphEngine as engine
 from ..model.distAPPNP import APPNP_ALPHA, APPNP_K
 from ..model.distGCNII import GCNII_ALPHA, GCNII_LAYERS, GCNII_THETA
+from ..model import ops
 from ..model.registry import MODELS, buffer_shape
 from ..manager.graphEngine import load_rank_layout
 from . import checkpoint as ckpt
@@ -32,6 +35,29 @@ RUNING_MODE = ["Vanilla", "AdaQP", "AdaQP-q", "AdaQP-p"]
 QUNAT_PARA_MAP: Dict[str, Tuple[str, bool]] = {"Vanilla": ("full", False), "AdaQP": ("quant", True),
                                                "AdaQP-q": ("quant", False), "AdaQP-p": ("full", True)}
 GAT_HEADS = 4          # default of the yaml `model: gat_heads`
+# run-time flags of Correct & Smooth -> cs_params arguments (None: the default)
+CS_FLAGS = {"cs_correct_layers": "correct_layers", "cs_correct_alpha": "correct_alpha",
+            "cs_smooth_layers": "smooth_layers", "cs_smooth_alpha": "smooth_alpha", "cs_scale": "scale"}
+
+
+def exchange_key_dims(config: dict, key_dims: Optional[Dict[str, int]], cs: bool) -> Optional[Dict[str, int]]:
+    """The exchange's key table: the model's own `key_dims` (None: the reference keys of buffer_shape) and, with
+    Correct & Smooth, CS_KEY as wide as the output.  The Assigner and the checkpoints keep `key_dims`."""
+    if not cs:
+        return key_dims
+    base = key_dims if key_dims is not None else layer_key_dims(buffer_shape(config, None))
+    return with_cs_key(base, config["data"]["num_classes"])
+
+
+def cs_config(config: dict) -> Optional[CSParams]:
+    """The checked C&S parameters of the run (None: not requested).  C&S smooths softmax outputs, so a multilabel
+    dataset is refused."""
+    rt = config["runtime"]
+    if not rt.get("correct_and_smooth"):
+        return None
+    if config["data"]["is_multilabel"]:
+        raise ValueError(f"Correct & Smooth is defined on softmax outputs; dataset '{rt['dataset']}' is multilabel")
+    return cs_params(**{arg: rt[flag] for flag, arg in CS_FLAGS.items() if rt.get(flag) is not None})
 
 
 class Trainer(object):
@@ -67,9 +93,12 @@ class Trainer(object):
         if rt["checkpoint_every"] > 0 and not rt["checkpoint_dir"]:
             raise ValueError("checkpoint_every > 0 needs checkpoint_dir")
         self.resume_path, self.resume_epoch, self._partition_digest = None, 0, None
+        self.cs = cs_config(self.config)
         self.exp_path = f"{rt['exp_path']}/{dataset}/{rt['num_parts']}part/{rt['model_name']}"
         self.logger = setup_logger("trainer.log", rt["logger_level"], with_file=True)
         self._set_communicator()
+        if self.cs is not None and comm.ctx.transport != "p2p":
+            raise NotImplementedError("Correct & Smooth runs on the p2p transport only (not the CPU gloo plumbing mode)")
         self._set_engine()
         if comm.get_rank() == 0:
             os.makedirs(self.exp_path, exist_ok=True)
@@ -121,7 +150,8 @@ class Trainer(object):
     def _set_buffer(self):
         comm.ctx.init_buffer(buffer_shape(self.config, self.key_dims), engine.ctx.send_idx, engine.ctx.recv_idx,
                              engine.ctx.bit_type, total_send_idx=engine.ctx.total_send_idx,
-                             num_remote=engine.ctx.num_remove, key_dims=self.key_dims)
+                             num_remote=engine.ctx.num_remove,
+                             key_dims=exchange_key_dims(self.config, self.key_dims, self.cs is not None))
         self.spec.setup(engine.ctx, comm.ctx.comm_buffer.p2p)
 
     def run_fields(self) -> dict:
@@ -237,19 +267,47 @@ class Trainer(object):
             self.predict_metrics = [float(m[2 * k] / max(float(m[2 * k + 1]), 1.0)) for k in range(3)]
         return logits
 
+    def correct_and_smooth(self, logits: Tensor) -> Tensor:
+        """Correct & Smooth (DESIGN §16) of predict()'s [n_inner, C] logits with this rank's train labels (val and
+        test labels are never read); every rank calls it together.  Returns the smoothed probabilities and sets
+        `cs_metrics`, their global train / val / test argmax accuracy.  Needs `correct_and_smooth` in the run's
+        arguments, which adds the exchange key the steps use."""
+        if self.cs is None:
+            raise ValueError("correct_and_smooth() needs the run to be built with correct_and_smooth set")
+        eng = self.engine.ctx
+        y = torch.full((eng.num_inner,), -1, dtype=torch.int32, device=logits.device)
+        y[eng.train_mask] = eng.labels[eng.train_mask].to(torch.int32)
+        n_train = torch.LongTensor([eng.train_mask.numel()])
+        comm.all_reduce_sum(n_train)
+        with torch.no_grad():
+            probs = ops.correct_and_smooth(eng.graph, logits, y, self.cs, int(n_train.item()))
+        _check_exchange_status()
+        m = []
+        for mask in (eng.train_mask, eng.val_mask, eng.test_mask):
+            m.extend(float(x) for x in get_metrics(eng.labels[mask], probs[mask], False))
+        m = torch.tensor(m, dtype=torch.float64)
+        comm.all_reduce_sum(m)
+        self.cs_metrics = [float(m[2 * k] / max(float(m[2 * k + 1]), 1.0)) for k in range(3)]
+        return probs
+
     def save_predictions(self, out_dir: str, checkpoint: str = None) -> str:
         """predict(), then each rank writes `out_dir/shard{r}.npz` (`node_id`, `logits`) and rank 0 merges the
         shards from disk into `out_dir/predictions.npz`: `node_id` int64 [N] ascending, `logits` float32 [N, C]
-        and a JSON header with the checkpoint's epoch and the train / val / test metric."""
+        and a JSON header with the checkpoint's epoch and the train / val / test metric.  With Correct & Smooth the
+        file also holds `cs_probs` float32 [N, C] (correct_and_smooth of the logits, merged the same way) and the
+        header its parameters (`correct_and_smooth`) and accuracies (`cs_train`, `cs_val`, `cs_test`)."""
         rank, W = comm.get_rank(), comm.get_world_size()
         gid = engine.ctx.layout.inner_gid
         if not all(comm.gather_all(gid is not None)):
             raise ValueError("the partition files carry no original node ids (inner_gid): re-partition with "
                              "graph_partition.py or tools/convert_dgl_partition.py to write predictions by node id")
         logits = self.predict(checkpoint)
+        extra = {}
+        if self.cs is not None:
+            extra["cs_probs"] = self.correct_and_smooth(logits).cpu().numpy()
         os.makedirs(out_dir, exist_ok=True)
         np.savez(os.path.join(out_dir, f"shard{rank}.npz"), node_id=np.asarray(gid, np.int64),
-                 logits=logits.float().cpu().numpy())
+                 logits=logits.float().cpu().numpy(), **extra)
         comm.barrier()
         final = os.path.join(out_dir, "predictions.npz")
         if rank == 0:
@@ -259,10 +317,15 @@ class Trainer(object):
             header = {"checkpoint": self.predict_checkpoint, "epoch": int(self.predict_manifest["epoch"]),
                       "num_parts": W, "metric": "f1_micro" if self.config["data"]["is_multilabel"] else "accuracy",
                       **dict(zip(("train", "val", "test"), self.predict_metrics))}
+            merged = {}
+            if self.cs is not None:
+                header["correct_and_smooth"] = self.cs.as_dict()
+                header.update(zip(("cs_train", "cs_val", "cs_test"), self.cs_metrics))
+                merged["cs_probs"] = np.concatenate([s["cs_probs"] for s in shards])[order]
             tmp = os.path.join(out_dir, ".predictions.tmp.npz")
             with open(tmp, "wb") as f:
                 np.savez(f, node_id=ids[order], logits=np.concatenate([s["logits"] for s in shards])[order],
-                         header_json=np.frombuffer(json.dumps(header).encode("utf-8"), dtype=np.uint8))
+                         header_json=np.frombuffer(json.dumps(header).encode("utf-8"), dtype=np.uint8), **merged)
             os.replace(tmp, final)
         comm.barrier()
         comm.ctx.delete_buffer()

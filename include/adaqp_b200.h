@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define ADAQP_ABI_VERSION 8
+#define ADAQP_ABI_VERSION 9
 
 #define ADAQP_EINVAL (-1)   /* bad argument (bits not in {1,2,4,8}, negative size ...) */
 #define ADAQP_EALIGN (-2)   /* pointer alignment requirement violated */
@@ -268,6 +268,36 @@ int adaqp_appnp_prop_f32(const int64_t *indptr, const int64_t *seg_start, const 
                          int64_t ld1, const float *pre, const float *post, float scale, float alpha,
                          const float *tele, int64_t ldt, float *acc, int64_t lda, int32_t acc_mode, int accumulate,
                          int64_t row_begin, int64_t row_end, int32_t F, float *out, int64_t ldo, void *stream);
+
+/* --------------------------------------------------------------- Correct & Smooth (DESIGN §16; host mirror
+ * adaqp_b200/cs.py).  y is int32 per row: the row's label where it is fixed (a train row), else -1.  Bad arguments
+ * (C outside [1, 1024], a bad row range or shape, null pointers, lo > hi, a bad scale) return ADAQP_EINVAL before any
+ * CUDA call.
+ *
+ * One propagation step over whole CSR rows [row_begin, row_end) <= n_split, the sources of adaqp_appnp_prop_f32:
+ *   r[v] = (scale * post[v]) * sum_{u in N(v)} pre[u] x[u]  (+ alpha * tele[v] in clamp mode, tele != NULL)
+ *   post_mode 0 (clamp): out[v] = min(max(r[v], lo), hi)
+ *   post_mode 1 (fix)  : out[v] = fix[v] where y[v] >= 0 (no gather for that row), else r[v]; tele is not read
+ * tele / y / fix / out rows are indexed v - row_begin.  The sum and the epilogue's rounding are appnp_prop's: with
+ * lo = -inf and hi = +inf the clamp step is bitwise adaqp_appnp_prop_f32's teleport step.  No segments: a clamp or a
+ * fixed row cannot be applied to two partial sums. */
+int adaqp_cs_prop_f32(const int64_t *indptr, const int32_t *indices, const float *x0, int64_t ld0, int64_t n_split,
+                      const float *x1, int64_t ld1, const float *pre, const float *post, float scale, float alpha,
+                      const float *tele, int64_t ldt, const int32_t *y, const float *fix, int64_t ldf,
+                      int32_t post_mode, float lo, float hi, int64_t row_begin, int64_t row_end, int32_t F,
+                      float *out, int64_t ldo, void *stream);
+
+/* Set-up of rows [0, rows): yhat = softmax(z) (row maximum subtracted), e0 = onehot(y) - yhat where y >= 0 and 0
+ * elsewhere, and partials[b] = the float64 sum of |e0| over the rows CTA b handles (the grid is n_partials CTAs; the
+ * partials depend only on the input and n_partials). */
+int adaqp_cs_init_f32(const float *z, int64_t ldz, const int32_t *y, int64_t rows, int32_t C, float *yhat,
+                      int64_t ldy, float *e0, int64_t lde, double *partials, int32_t n_partials, void *stream);
+
+/* Combine of rows [0, rows): g0[v] = onehot(y[v]) where y >= 0, else yhat[v] + s[v] e[v] with, for autoscale != 0,
+ * s[v] = value / |e[v]|_1 (value = sigma >= 0; s[v] = 1 where |e[v]|_1 = 0 or s[v] > 1000, decided in float64), and
+ * for autoscale == 0 s[v] = value (a finite scale > 0). */
+int adaqp_cs_combine_f32(const float *yhat, int64_t ldy, const float *e, int64_t lde, const int32_t *y, int64_t rows,
+                         int32_t C, int32_t autoscale, double value, float *g0, int64_t ldg, void *stream);
 
 /* --------------------------------------------------------------- dense GEMM
  * C[M, N] = A[M, K] . Bt[N, K]^T (+ bias[N]) in fp32 on the Hopper tensor cores (wgmma) by 3xTF32 error-compensated

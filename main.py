@@ -20,7 +20,7 @@ FLAGS = [
 ]
 
 
-def parse():
+def parse(argv=None):
     p = argparse.ArgumentParser(description="distributed full graph training (H100-native hot path)")
     for flag, typ, default, text in FLAGS:
         p.add_argument(flag, type=typ, default=default, help=text)
@@ -46,7 +46,24 @@ def parse():
                         "with --predict_out: the checkpoint to predict from (default <checkpoint_dir>/best)")
     p.add_argument("--predict_out", type=str, default=None,
                    help="instead of training, write per-node predictions (logits by original node id) to this directory")
-    return p.parse_args()
+    p.add_argument("--correct_and_smooth", action="store_true",
+                   help="with --predict_out: also write Correct & Smooth probabilities (cs_probs), which propagate the "
+                        "train labels over the graph (single-label datasets only)")
+    p.add_argument("--cs_correct_layers", type=int, default=None, help="C&S correct steps K1 (default 50)")
+    p.add_argument("--cs_correct_alpha", type=float, default=None,
+                   help="C&S correct propagation weight alpha1 in [0, 1] (default 0.8); 1 = pure propagation, the "
+                        "reverse of --appnp_alpha, which is the teleport weight")
+    p.add_argument("--cs_smooth_layers", type=int, default=None, help="C&S smooth steps K2 (default 50)")
+    p.add_argument("--cs_smooth_alpha", type=float, default=None,
+                   help="C&S smooth propagation weight alpha2 in [0, 1] (default 0.8); 1 = pure propagation, the "
+                        "reverse of --appnp_alpha")
+    p.add_argument("--cs_scale", type=str, default=None,
+                   help="C&S error scale: `auto` (default; autoscale by the mean train error) or a number > 0 (fixed "
+                        "scale, the train rows' errors held at each correct step)")
+    args = p.parse_args(argv)
+    if args.correct_and_smooth and not args.predict_out:
+        p.error("--correct_and_smooth needs --predict_out")
+    return args
 
 
 if __name__ == "__main__":
